@@ -2,9 +2,9 @@
 """bench.py — proofs/s on the BASELINE.json workload (Groth16, BN254, domain 2^20 synthetic chain circuit).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--log-n 20] [--impl reference]
-                    [--workload groth16|plonk|fflonk] [--curve bn128|bls12381]
+                    [--workload groth16|plonk|fflonk] [--curve bn128|bls12381] [--dump-outputs DIR]
 
-One step = one proof.  N = 1: the whole prover on one B200.  N > 1 (torchrun, one rank per GPU): every MSM is sharded
+One step = one proof.  N = 1: the whole prover on one H100.  N > 1 (torchrun, one rank per GPU): every MSM is sharded
 by point range across the ranks (north star / SURVEY §8e) and the three A/B/C transform chains run on different ranks;
 the exchange steps run inside libsnarkb200.so over NCCL.  `value` is the sharded single-proof rate (strong scaling);
 `replicas` reports N independent provers beside it.
@@ -30,6 +30,10 @@ sys.path.insert(0, ROOT)
 
 import numpy as np  # noqa: E402
 
+# roofline fallback when no measured HBM bandwidth is supplied: NVIDIA's data-sheet figure, not a measurement
+HBM_DATASHEET_GBS = 3350.0
+HBM_DATASHEET_SRC = "H100 SXM data sheet, 3350 GB/s (not measured)"
+
 
 def parse():
     ap = argparse.ArgumentParser()
@@ -45,7 +49,28 @@ def parse():
     ap.add_argument("--witness-like", action="store_true", help="witness distribution of real circuits (SURVEY 8d): 50%% zeros, 25%% ones, 25%% uniform")
     ap.add_argument("--tune", action="append", default=[], help="experimental kernel-variant switch k=v (sb_set_tuning), e.g. 1=1 = legacy bucket reduction")
     ap.add_argument("--mode", default="shard", choices=["shard", "replicas"], help="N > 1: which number is `value` (the other one is reported beside it)")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's proof to DIR/proof.npy (GPU arm); inputs depend only on the arguments")
+    a = ap.parse_args()
+    if a.dump_outputs and a.impl == "reference":
+        ap.error("--dump-outputs applies to the GPU arm")
+    return a
+
+
+def dump_outputs(out_dir: str, arrays: dict) -> None:
+    """One float64 .npy per array: proof bytes (0..255) are exact in float64."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.asarray(a, dtype=np.float64))
+
+
+def gpu_info(index: int) -> dict:
+    """Name and power limit of the card: part of every number measured on it."""
+    try:
+        o = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i", str(index)],
+                           capture_output=True, text=True, timeout=10).stdout.strip().split(",")
+        return {"name": o[0].strip(), "power_limit_w": float(o[1])}
+    except Exception:
+        return {}
 
 
 # ------------------------------------------------------------------------------------------------ clocks sampler
@@ -127,7 +152,7 @@ def workload_config(L: int, world: int, witness_like: bool) -> dict:
     return {"workload": f"groth16 prove, BN254, synthetic chain R1CS, domain 2^{L} (nVars 2^{L}, {2 * ((1 << L) - 3) + 2} QAP coefficients); 4 G1 MSM + 1 G2 MSM of 2^{L} points, 6 NTT of 2^{L}",
             "curve": "bn128", "witness": "witness-like (50% zeros, 25% ones)" if witness_like else "uniform field elements (chain circuit)",
             "parallelism": f"one proof over {world} GPUs: MSM point-range shards, A/B/C transform chains on ranks 0..2, NCCL exchange inside the library" if world > 1 else "single GPU",
-            "l2_policy": "inputs larger than L2 (384 MiB of bases + 32 MiB witness per proof vs 126 MB L2)"}
+            "l2_policy": "inputs larger than L2 (384 MiB of bases + 32 MiB witness per proof vs 50 MB L2)"}
 
 
 # ------------------------------------------------------------------------------------------------ reference arm / cpu baseline
@@ -164,7 +189,7 @@ def run_reference(args):
         import bench_plonk
         return bench_plonk.run_reference(args)
     L = args.cpu_log_n or args.log_n
-    steps = max(1, min(args.steps, 2))
+    steps = max(1, args.steps)
     warm = 1 if args.warmup > 0 else 0
     dt, cores, proof = oracle_groth16(L, steps, warm)
     scale = (1 << args.log_n) / (1 << L)
@@ -268,6 +293,7 @@ def run_b200(args):
         # per-stage breakdown of the last e2e step (CUDA events on the library's stream)
         brk = {"h2d_witness": curve.last_ms(1), "device_total": curve.last_ms(0)}
         dt_res = timed(lambda: step(True), args.steps)
+        proof_last = proof.copy()
     clocks = cs.summary()
     replicas = None
     if world > 1:
@@ -318,20 +344,14 @@ def run_b200(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s"
+    hbm_peak = float(peaks.get("hbm_gbs", HBM_DATASHEET_GBS))
+    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else HBM_DATASHEET_SRC
     # multiply-equivalents per entry from the wide-MAC count (one 8-limb Montgomery multiply = 2*64 + 8 = 136 wide MACs, a
     # dual-product multiply = 3*64 + 8 = 200): G1 mixed add = 8 multiplies + 1 dual = 1288 MACs = 9.47; G2 = 16 duals + 4
     # multiplies = 3744 MACs = 27.53
     g1_mod = acc["g1_entries"] * (1288.0 / 136.0)
     g2_mod = acc["g2_entries"] * (3744.0 / 136.0)
     dom = "g2" if acc["g2_ms"] >= acc["g1_ms"] / max(acc["g1_launches"], 1) else "g1"
-    traffic = None
-    try:   # DRAM bytes per launch of the dominant kernel from the committed ncu --set full capture (profiles/)
-        tj = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        traffic = tj.get("k_accumulate_g2" if dom == "g2" else "k_accumulate_g1", {}).get("dram_bytes_per_launch")
-    except Exception:
-        pass
     if dom == "g2":
         k_ms, k_launch, k_entries, k_mod, base_b, name = acc["g2_ms"], acc["g2_launches"], acc["g2_entries"], g2_mod, 128, "k_accumulate<Fp2<BnFq>> (G2 bucket accumulation)"
     else:
@@ -355,14 +375,14 @@ def run_b200(args):
         "e2e": {"value": args.steps / dt_e2e, "unit": "proofs/s", "h2d_bytes_per_step": int(nwit * 32), "d2h_bytes_per_step": int(proof.size),
                 "ms_per_step": dt_e2e / args.steps * 1e3, "api": ("sb_groth16_prove_dist (pinned host witness on every rank, 1/N uploaded per rank -> affine proof bytes on rank 0's host)" if world > 1 else "sb_groth16_prove (pinned host witness -> affine proof bytes on host)")},
         "gpu_launches": int(l1 - l0),
-        "clocks": clocks,
+        "gpu": gpu_info(local), "clocks": clocks,
         "roofline": {"bound": "hbm", "kernel": name, "achieved": ach_gbs, "peak": hbm_peak, "unit": "GB/s", "frac": ach_gbs / hbm_peak if hbm_peak else None,
-                     "traffic": traffic, "peak_source": peak_src, "launch_ms": avg_ms, "algorithmic_bytes_per_launch": alg_bytes,
+                     "peak_source": peak_src, "launch_ms": avg_ms, "algorithmic_bytes_per_launch": alg_bytes,
                      "note": "integer-pipe bound kernel: see roofline_int; HBM fraction is low by construction"},
         "roofline_int": {"bound": "int32 IMAD pipe (modmul-bound roofline, SURVEY 8d)", "kernel": name, "achieved": ach_mod / 1e9, "unit": "G Fq-modmul/s",
                          "peak": peak_modmul / 1e9, "frac": ach_mod / peak_modmul if peak_modmul > 0 else None,
                          "peak_source": "sb_calibrate(1): four independent per-thread BN254 Fq Montgomery-multiply chains (IMAD.WIDE.U32.X issue-bound), measured on this GPU in this run",
-                         "imad_wide_per_s": peak_imad, "imad_wide_per_clk_per_sm": (peak_imad / 148.0 / (clocks["sm_mhz"] * 1e6)) if clocks.get("sm_mhz") else None,
+                         "imad_wide_per_s": peak_imad, "imad_wide_per_clk_per_sm": (peak_imad / torch.cuda.get_device_properties(local).multi_processor_count / (clocks["sm_mhz"] * 1e6)) if clocks.get("sm_mhz") else None,
                          "all_accumulate_kernels_frac": (all_mod / (all_ms * 1e-3)) / peak_modmul if (all_ms > 0 and peak_modmul > 0) else None},
         "breakdown_ms": brk, "accumulate": acc, "setup_s": t_setup, "replicas": replicas,
         "proof_sha256": ph,                      # same inputs => same bytes at every N
@@ -392,6 +412,8 @@ def run_b200(args):
         except Exception as e:  # the baseline is a report, never a reason to lose the GPU number
             line["cpu_baseline"] = {"error": str(e)}
     print(json.dumps(line))
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"proof": proof_last})
     pk.release()
     curve.terminate()
     if dist is not None:

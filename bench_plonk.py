@@ -1,4 +1,4 @@
-"""bench_plonk.py — BASELINE.json config #5: `plonk prove` / `fflonk prove` at domain 2^L on one B200 (bench.py --workload
+"""bench_plonk.py — BASELINE.json config #5: `plonk prove` / `fflonk prove` at domain 2^L on one H100 (bench.py --workload
 plonk|fflonk).  Same JSON contract as bench.py's Groth16 line.
 
 One step = one proof of the synthetic chain circuit (snarkjs_b200/synth.py: 2^L - 6 gates, ~n/4 additions on two dependency
@@ -18,7 +18,9 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import time
+import zlib
 
 import numpy as np
 
@@ -44,9 +46,9 @@ def _proof_bytes(proto: str, n8q: int) -> int:
 
 # ------------------------------------------------------------------------------------------------ CPU port (reference arm)
 def host_flow_lib(proto: str):
-    """tests/host/host_<proto>.cpp compiled with OpenMP (cached under tests/host/build/)."""
+    """tests/host/host_<proto>.cpp compiled with OpenMP, cached in the temporary directory (the tree may be read-only)."""
     src = os.path.join(ROOT, "tests", "host", f"host_{proto}.cpp")
-    out_dir = os.path.join(ROOT, "tests", "host", "build")
+    out_dir = os.path.join(tempfile.gettempdir(), f"snarkjs_b200_host_{os.getuid()}_{zlib.crc32(ROOT.encode()):08x}")   # one per tree
     os.makedirs(out_dir, exist_ok=True)
     so = os.path.join(out_dir, f"libhost{proto}_omp.so")
     deps = [src, os.path.join(ROOT, "tests", "host", "host_backend.h")] + [os.path.join(ROOT, "snarkjs_b200", "csrc", f) for f in
@@ -113,7 +115,7 @@ def run_reference(args):
     t0 = time.perf_counter()
     zkey, wit, ci = oracle_key(proto, cname, L)
     t_setup = time.perf_counter() - t0
-    steps = max(1, min(args.steps, 2))
+    steps = max(1, args.steps)
     warm = 1 if (args.warmup > 0 and L <= 16) else 0
     raw = None
     for _ in range(warm):
@@ -146,7 +148,7 @@ def run_b200(args):
     import snarkjs_b200
     from snarkjs_b200 import fflonk, plonk, synth
     from snarkjs_b200.curve import _ptr
-    from bench import ClockSampler, host_cores, proof_hash
+    from bench import HBM_DATASHEET_GBS, HBM_DATASHEET_SRC, ClockSampler, dump_outputs, gpu_info, host_cores, proof_hash
 
     proto, cname, L = args.workload, _curve_name(args), args.log_n
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -215,6 +217,7 @@ def run_b200(args):
         proof_e2e = proof.copy()
         l1 = curve.launch_count()
         dt_res = timed(lambda: step(True), args.steps)
+        proof_last = proof.copy()
     clocks = cs.summary()
     assert np.array_equal(proof, proof_e2e), "resident and e2e proofs differ"
     # per-class device times of the last proof (the flow runs on one stream: event-bracketed durations are per-kernel costs)
@@ -233,7 +236,7 @@ def run_b200(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
+    hbm_peak = float(peaks.get("hbm_gbs", HBM_DATASHEET_GBS))
     n32 = curve.n8q // 4
     # dominant kernel: G1 bucket accumulation over the PTau window table (8 B entry + one affine base per entry)
     alg_bytes = acc_entries * (8 + 2 * curve.n8q) / acc_launches
@@ -244,12 +247,6 @@ def run_b200(args):
     ach_mod = (acc_entries * mod_per_entry / acc_launches) / (avg_ms * 1e-3) if avg_ms > 0 else 0.0
     # integer-pipe peak for this base field: the calibrated BN254 rate scaled by the wide-MAC count of one multiply (2N^2 + N)
     peak_mod = peak_modmul_bn * (2 * 8 * 8 + 8) / (2 * n32 * n32 + n32)
-    traffic = None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        traffic = tj.get(f"k_accumulate_g1_{cname}", {}).get("dram_bytes_per_launch")
-    except Exception:
-        pass
     ns = curve
     pobj = mod.proof_to_object(ns, proof.tobytes())
     ph = proof_hash(pobj)
@@ -263,12 +260,12 @@ def run_b200(args):
         "ms_per_step": dt_res / args.steps * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": f"u32x8 scalar field / u32x{n32} base field (modular integers, 32-bit limbs)", "data": "synthetic",
         "config": {"workload": wl, "curve": cname, "gates": n - 6, "n_additions": int(pk.nAdditions), "parallelism": "single GPU" if world == 1 else f"{world} independent provers (replicas: the rounds are serialised by the transcript)",
-                   "l2_policy": "inputs larger than L2 (key %.1f GB in HBM, %d MiB witness per proof vs 126 MB L2)" % (zkey_len / 1e9, nwit * 32 >> 20)},
+                   "l2_policy": "inputs larger than L2 (key %.1f GB in HBM, %d MiB witness per proof vs 50 MB L2)" % (zkey_len / 1e9, nwit * 32 >> 20)},
         "e2e": {"value": world * args.steps / dt_e2e, "unit": "proofs/s", "h2d_bytes_per_step": int(nwit * 32), "d2h_bytes_per_step": int(proof.size),
                 "ms_per_step": dt_e2e / args.steps * 1e3, "api": f"sb_{proto}_prove (pinned host witness -> proof bytes on host)"},
-        "gpu_launches": int(l1 - l0), "launches_per_proof": int((l1 - l0) // max(args.steps, 1)), "clocks": clocks,
+        "gpu_launches": int(l1 - l0), "launches_per_proof": int((l1 - l0) // max(args.steps, 1)), "gpu": gpu_info(local), "clocks": clocks,
         "roofline": {"bound": "hbm", "kernel": kname, "achieved": ach_gbs, "peak": hbm_peak, "unit": "GB/s", "frac": ach_gbs / hbm_peak if hbm_peak else None,
-                     "traffic": traffic, "peak_source": "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s",
+                     "peak_source": "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else HBM_DATASHEET_SRC,
                      "launch_ms": avg_ms, "algorithmic_bytes_per_launch": alg_bytes, "note": "integer-pipe bound kernel: see roofline_int"},
         "roofline_int": {"bound": "int32 IMAD pipe (modmul-bound roofline, SURVEY 8d)", "kernel": kname, "achieved": ach_mod / 1e9, "unit": "G Fq-modmul/s",
                          "peak": peak_mod / 1e9, "frac": ach_mod / peak_mod if peak_mod > 0 else None,
@@ -296,6 +293,8 @@ def run_b200(args):
         except Exception as e:
             line["cpu_baseline"] = {"error": str(e)}
     print(json.dumps(line))
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"proof": proof_last})
     pk.release()
     curve.terminate()
     if dist is not None:

@@ -1,7 +1,7 @@
-/* snarkb200.h — C ABI of libsnarkb200.so, the B200 (sm_100a) backend for snarkjs' bulk curve operations.
+/* snarkb200.h — C ABI of libsnarkb200.so, the H100 (sm_90a) backend for snarkjs' bulk curve operations.
  *
  * Every entry point replaces one async method of the ffjavascript `curve` object that snarkjs' provers call
- * (SURVEY.md §8b).  Citations are into /root/reference/build/snarkjs.js (first bundled copy of
+ * (SURVEY.md §8b).  Citations are into snarkjs' build/snarkjs.js (first bundled copy of
  * ffjavascript@0.3.1) unless a src/ path is given.  INTEGRATION.md shows the N-API shim that binds them.
  *
  * Conventions

@@ -1,4 +1,4 @@
-// snarkb200.mjs — overrides the bulk methods of snarkjs' curve singleton with the B200 backend.
+// snarkb200.mjs — overrides the bulk methods of snarkjs' curve singleton with the CUDA backend.
 // Usage:  import { useB200 } from "./snarkb200.mjs";  await useB200("bn128");  await snarkjs.groth16.prove(zkey, wtns);
 // Not runnable in this repository's image (no Node.js); see INTEGRATION.md for the line-by-line rationale.
 import { createRequire } from "module";

@@ -1,5 +1,5 @@
 // snarkb200_napi.cc — N-API addon binding libsnarkb200.so's C ABI (include/snarkb200.h) for Node.js.
-// Not built for Node in this repository's image (no node / node-addon-api headers here or on the GPU box); it is the binding a
+// Not built for Node by this repository's build or tests (they need no node / node-addon-api headers); it is the binding a
 // snarkjs maintainer adds, see INTEGRATION.md.  Build with node-gyp (binding.gyp next to this file).  What IS checked here:
 // tests/test_abi.py compiles this file against an in-process stand-in for the N-API classes it uses
 // (tests/host/napi_stub/napi.h), links it against the real libsnarkb200.so and drives it (tests/host/napi_shim_check.cpp).

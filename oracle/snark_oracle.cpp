@@ -7,7 +7,7 @@
 //
 // The reference (iden3/snarkjs 0.7.6) has no native code: its arithmetic lives in the
 // npm dependencies ffjavascript@0.3.1 -> wasmcurves@0.2.2 (WASM generated at run time),
-// absent from node_modules but bundled verbatim into /root/reference/build/snarkjs.js.
+// absent from node_modules but bundled verbatim into snarkjs' build/snarkjs.js.
 // Each function below cites the bundle lines (first copy, 1-17660) it restates.
 // There is no JS/WASM runtime in the build container, so the reference cannot be run
 // here; parity is pinned instead against the reference-produced bytes embedded in the

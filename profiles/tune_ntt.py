@@ -1,4 +1,4 @@
-"""Primitive-level timings on one B200 (BASELINE.json configs #2 and #3): BN254 G1/G2 MSM at 2^20 and Fr NTT/iNTT at
+"""Primitive-level timings on one GPU (BASELINE.json configs #2 and #3): BN254 G1/G2 MSM at 2^20 and Fr NTT/iNTT at
 2^20..2^24, device-resident (CUDA events inside the library) and through the host-buffer C ABI calls."""
 import ctypes, json, os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -97,7 +97,7 @@ EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 
 
 def build(verbose: bool = False) -> str:
-    """Compile libsnarkb200.so in-tree for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile libsnarkb200.so in-tree for sm_90a (nvcc cross-compiles without a GPU)."""
     cmd = ["make", "-C", os.path.join(_HERE, "csrc"), "-j8"]
     subprocess.check_call(cmd, stdout=None if verbose else subprocess.DEVNULL)
     return LIB_PATH

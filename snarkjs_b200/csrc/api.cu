@@ -481,7 +481,7 @@ template <class PR> static void fr_neg_mul_bytes(const uint8_t* r, const uint8_t
 // ================================================================================================================
 extern "C" {
 
-const char* sb_version(void) { return "snarkb200 0.2 (sm_100a)"; }
+const char* sb_version(void) { return "snarkb200 0.2 (sm_90a)"; }
 int sb_comm_destroy(sb_ctx* c);
 
 int sb_create(int curve, int device_id, sb_ctx** out) {

@@ -29,7 +29,7 @@ __global__ void __launch_bounds__(256) k_calib_modmul(uint32_t* out, int iters) 
     F r = F::add(F::add(a, b), F::add(c, d));
     out[blockIdx.x * blockDim.x + threadIdx.x] = r.v[0] ^ r.v[7];
 }
-// ---- FP64 exploration (round-2 planning): B200 has a full-rate FP64 pipe that the integer kernels leave idle.  A 52-bit
+// ---- FP64 exploration: the GPU has a full-rate FP64 pipe that the integer kernels leave idle.  A 52-bit
 // limb product needs two DFMAs (high and low half, Emmart's fma_rz trick), one DADD and two 64-bit integer adds.
 __global__ void __launch_bounds__(256) k_calib_dfma(double* out, int iters) {
     double acc[8];

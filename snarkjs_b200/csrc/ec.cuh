@@ -35,7 +35,7 @@ template <class P> struct Fp2 {
     // force-inlined variants for the hot bucket-accumulation loop (everything else calls the out-of-line ones to keep
     // code size and compile time down)
     SB_HD static Fp2 mul_i(const Fp2& x, const Fp2& y) {
-#if defined(__CUDA_ARCH__) && defined(SB_FP2_LAZY)   // measured slower on B200 (8.3 vs 7.0 ms per 2^20 G2 accumulation): register pressure
+#if defined(__CUDA_ARCH__) && defined(SB_FP2_LAZY)   // off by default: fewer MACs, but more live registers in the G2 accumulation
         return mul_lazy(x, y);          // 5 N^2 wide MACs
 #endif
         if constexpr (B::HAS_MUL2) {

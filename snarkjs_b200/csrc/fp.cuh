@@ -1,4 +1,4 @@
-// fp.cuh — prime-field arithmetic for sm_100a: N x 32-bit limbs, Montgomery form, R = 2^(32N).
+// fp.cuh — prime-field arithmetic for sm_90a: N x 32-bit limbs, Montgomery form, R = 2^(32N).
 //
 // Replaces wasmcurves' build_f1m (reference build/snarkjs.js:2861-3830; mul 3072-3273) on the GPU.
 // The reference multiplies by product scanning with 64-bit WASM accumulators; here the multiply is a

@@ -1,4 +1,4 @@
-// msm.cuh — Pippenger multi-scalar multiplication on one B200 (templated on the coordinate field).
+// msm.cuh — Pippenger multi-scalar multiplication on one GPU (templated on the coordinate field).
 //
 // Replaces ffjavascript engine_multiexp (_multiExp/_multiExpChunk, reference build/snarkjs.js:14517-14669)
 // and wasmcurves build_multiexp (g?m_multiexpAffine_chunk 5542-5695, _getChunk 5471-5540,
@@ -647,8 +647,8 @@ struct MsmSorted {
     // per bucket the runs of equal head keys outgrow k_fold_short's parallel path).  The actual value is chosen on the
     // device (k_count_valid, counts[MSM_COUNTS_SEG]) once the number of valid entries M is known: every thread does the same
     // work, so the kernel time is waves x seg, and seg = ceil(M / (k * resident threads)) makes the grid exactly k full waves
-    // of the 148 SMs instead of k - 1 waves and a fraction (applied for k <= 3: shards of a multi-GPU proof, small MSMs;
-    // measured on the 2-GPU shards: G1 accumulation -7.5 %, G2 -10.6 %; with more waves the effect vanishes).  seg_lo = the smallest value the device may pick (grid and
+    // of the SMs instead of k - 1 waves and a fraction (applied for k <= 3: shards of a multi-GPU proof, small MSMs; with
+    // more waves the effect vanishes).  seg_lo = the smallest value the device may pick (grid and
     // head-buffer sizing on the host).
     uint32_t seg_lo = MSM_SEG;
 };
@@ -673,9 +673,8 @@ int msm_buckets_impl(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& s
 
 // Entry: optional batched-affine pairing rounds (msm_pair.cuh) shrink the entry list first, then the segmented XYZZ
 // pipeline runs on what is left.  EXPERIMENTAL, off by default (enable with sb_set_tuning(4, 2), cap the rounds with
-// sb_set_tuning(5, R)): measured on B200 at 2^20 the rounds run the integer pipe at 40-60 % (scan + shared inversion +
-// two gather passes) against 93 % / 71 % for the XYZZ accumulation, which cancels the 6-vs-10 modmul advantage
-// (G1 3.7 ms vs 3.4 ms per MSM, G2 11.6 ms vs 11.8 ms; profiles/README.md).
+// sb_set_tuning(5, R)): the rounds (scan + shared inversion + two gather passes) keep the integer pipe less busy than
+// the XYZZ accumulation does, which cancels their 6-vs-10 modmul advantage.
 template <class F>
 int msm_buckets(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& scratch, cudaStream_t stream,
                 XYZZ<F>* d_wsum, MsmLaunchStats* stats, cudaStream_t tail_stream = nullptr, cudaEvent_t ev_acc = nullptr) {
@@ -787,20 +786,21 @@ int msm_buckets_impl(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& s
                 else switch (g_msm_tuning[0]) {
                 case 3: k_accumulate<F, 3><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;
                 case 4: k_accumulate<F, 4><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;
-                default: k_accumulate<F, 2><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;   // measured best: 8.0 ms vs 8.5 (2^20 G2)
+                default: k_accumulate<F, 2><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;   // H100 (400 W), 2^20 G2: 7.6 ms vs 8.3 (3), 9.2 (4), 8.3 (lane pair)
                 }
             } else if constexpr (sizeof(F) > 32) {
                 // 12-limb base field (BLS12-381 G1).  At 4 CTAs/SM the 128-register cap spills ~50 words of the mixed addition
-                // (ptxas: 218 B spill stores / 188 B loads); 3 CTAs/SM (168 registers) and 2 (190) do not spill.  Measured on the
-                // B200 (PLONK 2^18, nine accumulations): 2 CTAs/SM 15.8 ms, 4 CTAs/SM 16.7 ms, 3 CTAs/SM 19.3 ms
-                // (profiles/ab_r2_summary.txt) -> 2 is the default; sb_set_tuning(10, 3 | 4) selects the others.
+                // (ptxas, sm_90a: 184 B spill stores / 132 B loads); 3 CTAs/SM (167 registers) and 2 (182) do not spill.  Measured on an
+                // H100 at 400 W (PLONK BLS12-381 2^18, nine accumulations): 2 CTAs/SM 15.5 ms, 4 CTAs/SM 16.7 ms, 3 CTAs/SM 19.1 ms
+                // -> 2 is the default; sb_set_tuning(10, 3 | 4) selects the others.
                 switch (g_msm_tuning[8]) {
                 case 4: k_accumulate<F, 4><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;
                 case 3: k_accumulate<F, 3><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;
                 default: k_accumulate<F, 2><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;
                 }
             } else {
-                // 8-limb base field (BN254 G1): 122 registers at 4 CTAs/SM, no spills; sb_set_tuning(12, 3 | 2) = lower-occupancy builds
+                // 8-limb base field (BN254 G1): 116 registers at 4 CTAs/SM, no spills; sb_set_tuning(12, 3 | 2) = lower-occupancy
+                // builds (H100 at 400 W, 2^20 Groth16: all three within 1 %)
                 switch (g_msm_tuning[10]) {
                 case 3: k_accumulate<F, 3><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;
                 case 2: k_accumulate<F, 2><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;

@@ -139,7 +139,7 @@ int msm_sort_entries(const uint8_t* d_scalars, uint32_t sbytes, uint64_t n, MsmG
     if (adaptive) { const uint64_t avg = nbuckets ? total / nbuckets : 0; while (T < 256 && avg > 2ull * T) T <<= 1; }
     if (g_msm_tuning[7] > 0) T = (uint32_t)g_msm_tuning[7];
     static int sm_count = 0;
-    if (!sm_count) { int dev = 0; cudaGetDevice(&dev); if (cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sm_count <= 0) sm_count = 148; }
+    if (!sm_count) { int dev = 0; cudaGetDevice(&dev); if (cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sm_count <= 0) sm_count = 132; }
     const uint64_t wave = adaptive ? (uint64_t)sm_count * 4 * MSM_ACC_THREADS : 0;     // 4 CTAs of 128 threads per SM (2 for the extension-field kernels: same fit)
     const uint32_t seg_lo = adaptive ? (T == (uint32_t)MSM_SEG ? 16u : T / 2) : T;
     k_count_valid<<<1, 1, 0, stream>>>(kb.Current(), total, counts, T, seg_lo, wave); launches++;

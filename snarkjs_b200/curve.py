@@ -1,7 +1,7 @@
 """Host-side mirror of the ffjavascript `curve` object for the bulk methods snarkjs' provers call
 (SURVEY.md §8b): same method names, argument meaning and error strings as the reference
 (build/snarkjs.js:14666-14668 multiExpAffine, 15101-15107 fft/ifft, 14273-14384 batchApplyKey,
-12895-12896 batchTo/FromMontgomery), executed on the B200 through the C ABI.
+12895-12896 batchTo/FromMontgomery), executed on the GPU through the C ABI.
 
 Buffers are bytes / bytearray / numpy uint8 arrays (the reference takes Uint8Array or BigBuffer); results are
 numpy uint8 arrays (fresh buffers, like the reference's).  Methods are synchronous here — the N-API shim

@@ -1,4 +1,4 @@
-"""fflonk.prove on the B200 — host-side mirror of src/fflonk_prove.js:51-267.
+"""fflonk.prove on the GPU — host-side mirror of src/fflonk_prove.js:51-267.
 
 ProvingKey(zkey) puts the fflonk key in HBM once (sb_fflonk_load); prove() runs the five rounds on the device
 (sb_fflonk_prove) and returns the {polynomials: {C1, C2, W1, W2}, evaluations: {ql .. t2w, inv}} object and the

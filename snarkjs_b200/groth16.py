@@ -1,4 +1,4 @@
-"""groth16.prove on the B200 — host-side mirror of src/groth16_prove.js:28-144.
+"""groth16.prove on the GPU — host-side mirror of src/groth16_prove.js:28-144.
 
 Two routes, same results:
   * prove(...)            fused path: sb_groth16_load once per zkey + sb_groth16_prove per witness (QAP, NTTs, MSMs all

@@ -1,4 +1,4 @@
-"""plonk.prove on the B200 — host-side mirror of src/plonk_prove.js:47-165.
+"""plonk.prove on the GPU — host-side mirror of src/plonk_prove.js:47-165.
 
 ProvingKey(zkey) puts the PLONK key in HBM once (sb_plonk_load); prove() runs the five rounds on the device
 (sb_plonk_prove: plonk.cuh kernels + NTT + table-mode MSM, transcript hashing on the host) and returns the same

@@ -12,7 +12,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def _gpu_available() -> bool:
@@ -31,12 +31,12 @@ def _gpu_available() -> bool:
 
 def pytest_collection_modifyitems(config, items):
     """`pytest tests` on a host without CUDA skips the gpu-marked parity tests instead of erroring in their fixtures.
-    (`-m gpu` on the B200 box runs them; there a missing library or device is a hard failure, not a skip.)"""
+    (`-m gpu` on an H100 runs them; there a missing library or device is a hard failure, not a skip.)"""
     gpu_items = [it for it in items if it.get_closest_marker("gpu")]
     if not gpu_items or "gpu" in (config.getoption("-m") or "").replace("not gpu", ""):
         return
     if not _gpu_available():
-        skip = pytest.mark.skip(reason="no CUDA device: gpu parity tests run on the B200 box")
+        skip = pytest.mark.skip(reason="no CUDA device: gpu parity tests run on an H100")
         for it in gpu_items:
             it.add_marker(skip)
 

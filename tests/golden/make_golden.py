@@ -1,9 +1,7 @@
 #!/usr/bin/env python
 """Extracts reference-produced golden vectors from the reference's committed fixtures
-(/root/reference/test/**) into small .npz files under tests/golden/.
-
-Run in the build container only (the GPU box has no /root/reference):
-    python tests/golden/make_golden.py
+(test/** of a snarkjs checkout) into small .npz files under tests/golden/.  Needs the checkout, no GPU:
+    SNARKJS_DIR=<snarkjs checkout> python tests/golden/make_golden.py
 
 What is extracted (all bytes below were written by the reference's own Fr.fft /
 G.multiExpAffine / G.ifft — SURVEY.md fact 6 / Appendix B):
@@ -27,7 +25,7 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 from oracle import oracle as O  # noqa: E402
 
-REF = "/root/reference/test"
+REF = os.path.join(os.environ.get("SNARKJS_DIR", "snarkjs"), "test")
 
 
 def u8(b):

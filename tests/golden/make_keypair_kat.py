@@ -1,12 +1,12 @@
 """Extracts the reference's only hard-coded known-answer vectors (test/keypar_test.js:20-119: three (g1_s, g1_sx, g2_spx)
 triples of a powers-of-tau public key and the challenge they were made for) into tests/golden/keypair_kat.json.
-Run in the build container, where /root/reference exists; the GPU box and the tests only see the JSON."""
+Needs a snarkjs checkout (SNARKJS_DIR=<checkout> python tests/golden/make_keypair_kat.py); the tests only read the JSON."""
 import json
 import os
 import re
 
-SRC = "/root/reference/test/keypar_test.js"
 HERE = os.path.dirname(os.path.abspath(__file__))
+SRC = os.path.join(os.environ.get("SNARKJS_DIR", "snarkjs"), "test", "keypar_test.js")
 
 
 def main():

@@ -1,5 +1,5 @@
 // napi.h — a stand-in for the subset of node-addon-api that integration/napi/snarkb200_napi.cc uses.  TEST INFRASTRUCTURE:
-// there is no Node.js (and no node-addon-api) in this image or on the GPU box, so the shim cannot be built for its real
+// there is no Node.js (and no node-addon-api) in the build and test environment, so the shim cannot be built for its real
 // host.  This header gives the same class and method names a small in-process implementation (values are tagged C++
 // objects, an AsyncWorker runs Execute() and its completion callback synchronously inside Queue()), so that the shim
 // compiles against the declared signatures, links against the real libsnarkb200.so and can be driven by
@@ -98,7 +98,9 @@ class AsyncWorker {
     virtual ~AsyncWorker() {}
     Napi::Env Env() const { return Napi::Env(); }
     void SetError(const std::string& m) { err_ = m; failed_ = true; }
-    void Queue() { Execute(); if (failed_) OnError(Error::New(Env(), err_)); else OnOK(); delete this; }
+    // Node deletes a worker on the event loop, after the binding that queued it has returned (the binding may still read
+    // the worker's members); here the previous worker is deleted on the next Queue() and the last one at exit.
+    void Queue() { Execute(); if (failed_) OnError(Error::New(Env(), err_)); else OnOK(); static std::unique_ptr<AsyncWorker> last; last.reset(this); }
  protected:
     virtual void Execute() = 0;
     virtual void OnOK() {}

@@ -101,7 +101,7 @@ def test_napi_shim_compiles_links_and_reports_no_device(tmp_path):
     an in-process stand-in for the N-API classes it uses (tests/host/napi_stub/napi.h), linked against the real
     libsnarkb200.so and driven by tests/host/napi_shim_check.cpp: every C-ABI call of the shim type-checks against
     include/snarkb200.h, all sixteen functions snarkb200.mjs calls are exported, and createContext surfaces the library's
-    no-device error on this machine (on a GPU box the same driver pushes an NTT and an MSM through the AsyncWorkers)."""
+    no-device error without a GPU (with a GPU the same driver pushes an NTT and an MSM through the AsyncWorkers)."""
     import subprocess
     from snarkjs_b200 import _native
     exe = str(tmp_path / "napi_shim_check")

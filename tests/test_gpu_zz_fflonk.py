@@ -5,7 +5,6 @@ import json
 
 import pytest
 
-# All cases have a recorded green hardware run (GPUTEST_r01.json, driver run at the end of round 1).
 pytestmark = pytest.mark.gpu
 
 BLINDERS = [0x6000 + 32452843 * i for i in range(9)]

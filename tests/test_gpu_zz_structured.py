@@ -1,6 +1,5 @@
 """GPU: Groth16 proofs from sb_groth16_prove on structured synthetic keys (oracle/synth_setup.py) equal the oracle's and
-VERIFY under the pairing check — on BN254 and on BLS12-381, where the reference ships no fixtures (green on the B200 since
-the round-1 driver run, GPUTEST_r01.json)."""
+VERIFY under the pairing check — on BN254 and on BLS12-381, where the reference ships no fixtures."""
 import pytest
 
 pytestmark = pytest.mark.gpu
