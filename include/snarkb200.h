@@ -200,18 +200,14 @@ double sb_last_stat(sb_ctx* ctx, int which);
 /* integer-pipe calibration on this device: what = 0 -> IMAD.WIDE.U32 per second, 1 -> register-resident BN254 Fq
  * Montgomery multiplies per second (the modmul-bound roofline denominators, SURVEY.md §8d). */
 double sb_calibrate(sb_ctx* ctx, int what);
-/* kernel-variant selection for experiments and profiling (process-wide; every variant computes the same bytes):
- *   0  minBlocksPerSM of the extension-field (G2) bucket accumulation (2 default, 3, 4)
- *   1  bucket reduction: 0 axis sums + warp-shuffle weighted sums (default), 1 legacy running sums, 2 hierarchical running sums
+/* process-wide switches for profiling and tests (every setting computes the same bytes); SB_ERR_ARG for any other key:
+ *   1  bucket reduction: 0 = axis sums + warp-shuffle weighted sums (default), 1 = running sums (k_reduce, the path for
+ *      windows of more than 2^20 buckets)
  *   2  1 = run every stream of a prove call serialised on one stream (per-kernel-class timing, sb_last_stat 8..15)
  *   3  1 = ignore the precomputed window tables (plain windowed Pippenger on the raw bases)
- *   4  2 = batched-affine pairing rounds before the accumulation;  5 = cap on their number (-1: also disables the adaptive
- *      entries-per-thread choice)
- *   6  log2 of the points per MSM chunk (test hook)        7  log2 of the largest NTT tile (10..12)
- *   8  0 = no pinned staging of pageable host buffers       9  forced sorted entries per accumulation thread (0 = adaptive)
- *   10 minBlocksPerSM of the 12-limb base-field (BLS12-381 G1) accumulation (2 default, 3, 4)
- *   12 minBlocksPerSM of the 8-limb base-field (BN254 G1) accumulation (4 default, 3, 2)
- *   11 lane-pair G2 accumulation (each point spread over two lanes, ec.cuh Fp2L): 0 = off, 3 / 4 = its minBlocksPerSM
+ *   6  log2 of the points per MSM chunk (test hook; 0 = default)
+ *   7  log2 of the largest NTT tile (10..12)
+ *   8  0 = no pinned staging of pageable host buffers
  * The Python mirror applies SB_TUNE="key=value,..." from the environment when it loads the library. */
 int sb_set_tuning(int key, int value);
 /* synthetic bases for tests/benchmarks: chunks of 4096 points P_{c,j} = (k0(seed, c) + j*kd(seed)) * G, affine Montgomery, computed

@@ -135,8 +135,8 @@ def lib():
             fn.restype = res
             fn.argtypes = args
         _lib = L
-        # experiment selection without code changes: SB_TUNE="key=value,key=value" -> sb_set_tuning (kernel variants only:
-        # every variant computes the same bytes)
+        # profiling and test switches without code changes: SB_TUNE="key=value,key=value" -> sb_set_tuning (keys in
+        # include/snarkb200.h; every setting computes the same bytes, an unknown key is an error)
         for kv in filter(None, os.environ.get("SB_TUNE", "").split(",")):
             k, v = kv.split("=")
             if L.sb_set_tuning(int(k), int(v)) != 0:

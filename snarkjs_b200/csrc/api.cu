@@ -351,10 +351,15 @@ void prof_end(sb_ctx* c) {
     c->stats.ev = nullptr; c->stats.used = 0;
 }
 
+// Process-wide switches of sb_set_tuning (key 1 is g_msm_force_reduce, msm.cuh).
+int g_serial_prove = 0;     // key 2: run every stream of a Groth16 prove call serialised on one stream (per-kernel-class timing)
+int g_no_tables = 0;        // key 3: ignore the precomputed window tables
+int g_msm_chunk_log = 0;    // key 6: log2 of the points per MSM chunk, 0 = 23 (a test hook)
+
 // Precomputed window tables (msm.cuh k_precompute).  Built for sets of >= 2^12 points whose table index fits the
-// 31-bit entry value; g_msm_tuning[3] != 0 disables them (plain windowed Pippenger on the raw bases).
+// 31-bit entry value; g_no_tables disables them (plain windowed Pippenger on the raw bases).
 bool want_precomp(sb_ctx* c, uint64_t n) {
-    if (g_msm_tuning[3] != 0 || n < (1ull << 12)) return false;
+    if (g_no_tables || n < (1ull << 12)) return false;
     MsmGeom g = msm_geometry_precomp(n, 32, c->fr_bits);
     return (uint64_t)g.W * n < (1ull << 31);
 }
@@ -379,7 +384,7 @@ float elapsed(sb_ctx* c, int a, int b) { float ms = 0; cudaEventElapsedTime(&ms,
 // ------------------------------------------------------------------------------------------------------------
 int msm_dev_accumulate(sb_ctx* c, const GroupOps& G, const void* d_bases, const uint8_t* d_scalars, uint32_t sbytes, uint64_t n,
                        uint8_t* acc_xyzz, const MsmGeom* gp = nullptr, uint64_t first = 0) {
-    const uint64_t MAXC = 1ull << (g_msm_tuning[6] > 0 ? g_msm_tuning[6] : 23);   // points per MSM chunk (tuning key 6: test hook)
+    const uint64_t MAXC = 1ull << (g_msm_chunk_log > 0 ? g_msm_chunk_log : 23);   // points per MSM chunk
     for (uint64_t off = 0; off < n; off += MAXC) {
         uint64_t cn = std::min(MAXC, n - off);
         MsmGeom g = msm_geometry(cn, sbytes, c->fr_bits);
@@ -714,13 +719,15 @@ int sb_fr_root(sb_ctx* c, int what, uint8_t out[32]) { SB_LOCK(c);
 }
 
 int sb_set_tuning(int key, int value) {
-    if (key == 8) { g_stage_enabled = value; return 0; }                                                      // pinned staging of pageable buffers
-    if (key == 7) { if (value < 10 || value > 12) return SB_ERR_ARG; g_ntt_tile_log = value; return 0; }   // NTT tile size
-    if (key == 9) { g_msm_tuning[7] = value; return 0; }                                                      // forced entries per accumulation thread (0 = adaptive)
-    if (key == 12) { g_msm_tuning[10] = value; return 0; }                                                    // minBlocksPerSM variant of the 8-limb base-field accumulation (BN254 G1): 4 default, 3, 2
-    if (key == 11) { g_msm_tuning[9] = value; return 0; }                                                     // lane-pair G2 accumulation (k_accumulate_pair): 0 = off, 3 / 4 = minBlocksPerSM
-    if (key == 10) { g_msm_tuning[8] = value; return 0; }                                                     // minBlocksPerSM variant of the 12-limb base-field accumulation (BLS12-381 G1)
-    if (key < 0 || key >= 7) return SB_ERR_ARG; g_msm_tuning[key] = value; return 0;
+    switch (key) {
+    case 1: if (value != 0 && value != 1) return SB_ERR_ARG; g_msm_force_reduce = value; return 0;   // bucket reduction
+    case 2: g_serial_prove = value; return 0;                                                           // serialised prove call
+    case 3: g_no_tables = value; return 0;                                                              // no window tables
+    case 6: g_msm_chunk_log = value; return 0;                                                          // MSM chunk size
+    case 7: if (value < 10 || value > 12) return SB_ERR_ARG; g_ntt_tile_log = value; return 0;         // NTT tile size
+    case 8: g_stage_enabled = value; return 0;                                                          // pinned staging of pageable buffers
+    default: return SB_ERR_ARG;
+    }
 }
 double sb_last_stat(sb_ctx* c, int which) { SB_LOCK(c); return (c && which >= 0 && which < 16) ? c->stat[which] : 0.0; }
 double sb_calibrate(sb_ctx* c, int what) { SB_LOCK(c); if (!c) return -1; cudaSetDevice(c->device); return calibrate(what, c->stream); }
@@ -1137,7 +1144,7 @@ static int groth16_device(sb_ctx* c, Groth16Key* k, const uint8_t* witness, uint
     uint8_t* pA = partials; uint8_t* pB1 = pA + G1.xyzz_bytes; uint8_t* pC = pB1 + G1.xyzz_bytes; uint8_t* pH = pC + G1.xyzz_bytes; uint8_t* pB2 = pH + G1.xyzz_bytes;
     memset(partials, 0, 4 * G1.xyzz_bytes + G2.xyzz_bytes);
     std::vector<uint8_t> sA(G1.xyzz_bytes, 0), rB1(G1.xyzz_bytes, 0);
-    const uint64_t MAXC = 1ull << (g_msm_tuning[6] > 0 ? g_msm_tuning[6] : 23);   // points per MSM chunk (tuning key 6: test hook)
+    const uint64_t MAXC = 1ull << (g_msm_chunk_log > 0 ? g_msm_chunk_log : 23);   // points per MSM chunk
     // a key loaded with sb_groth16_load_sharded only holds its own ranges: local indexing
     const bool local = k->n_shards > 1;
     if (local && (shard != k->shard || n_shards != k->n_shards)) return fail(c, SB_ERR_ARG, "proving key was loaded for a different shard");
@@ -1148,8 +1155,8 @@ static int groth16_device(sb_ctx* c, Groth16Key* k, const uint8_t* witness, uint
         // Overlapped pipeline: the witness is sorted once (A, B1, B2 and C all multiply it, :84-97); the four bucket
         // pipelines run on their own streams so that the latency-bound tails (fold cascade, bucket reduction) of one
         // MSM hide under the throughput-bound accumulation of the next; the H scalars (QAP/NTT chain) are produced
-        // concurrently on the main stream.  g_msm_tuning[2] != 0 serialises everything on one stream (profiling).
-        const bool serial = g_msm_tuning[2] != 0;
+        // concurrently on the main stream.  g_serial_prove serialises everything on one stream (profiling).
+        const bool serial = g_serial_prove != 0;
         cudaStream_t s0 = c->stream;
         // schedule: main stream  : H2D, sort(witness), acc B2, acc A, acc B1, acc C, [join NTT chain], acc H
         //           aux[5] (hi)  : QAP -> iNTT -> coset NTT -> [exchange] -> joinABC -> sort(H scalars)

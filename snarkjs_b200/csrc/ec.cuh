@@ -69,96 +69,6 @@ template <class P> struct Fp2 {
     }
 };
 
-// Fp2 spread over a lane pair: the even lane of the pair holds c0, the odd lane c1, so a point costs each thread half the
-// registers of Fp2 (the G2 bucket accumulation needs 252 registers per thread with Fp2 and runs 2 warps per scheduler;
-// with Fp2L it has the register footprint of the G1 kernel).  Additions are local; a multiply fetches the partner's
-// components with two 8/12-limb shuffles and is one dual-product Montgomery multiply per lane:
-//     even lane: c0 = x.a*y.a + x.b*(-y.b)        odd lane: c1 = x.b*y.a + x.a*y.b
-// written branch-free as mul2(x.mine, P, x.other, Q) with (P, Q) = (y.mine, -y.other) on the even and (y.other, y.mine) on the odd lane.
-// Squaring is one plain multiply per lane: (a + b)(a - b) on the even lane, (a + a)*b on the odd lane.  Predicates
-// (is_zero, ==) are combined over the pair with a vote, so both lanes always take the same branch; every warp primitive
-// uses the pair's own mask, so different pairs of a warp may diverge freely.  Device-only in the product; with
-// SB_PAIR_HOST_EMULATE the three pair primitives become calls into the test harness (tests/host/host_pair_check.cpp runs
-// the two lanes as two host threads in lockstep), so the same template code is checked against Fp2 without a GPU.
-#if !defined(__CUDA_ARCH__) && defined(SB_PAIR_HOST_EMULATE)
-bool sb_pair_odd();
-void sb_pair_exchange(const uint32_t* mine, uint32_t* others, int n);
-bool sb_pair_all(bool p);
-#endif
-template <class P> struct Fp2L {
-    typedef Fp<P> B;
-    static constexpr bool HAS_MUL2 = false;
-    B m;
-    SB_HD static unsigned pmask() {
-#ifdef __CUDA_ARCH__
-        return 3u << (threadIdx.x & 30u);
-#else
-        return 0;
-#endif
-    }
-    SB_HD static bool odd() {
-#ifdef __CUDA_ARCH__
-        return (threadIdx.x & 1u) != 0;
-#elif defined(SB_PAIR_HOST_EMULATE)
-        return sb_pair_odd();
-#else
-        return false;
-#endif
-    }
-    SB_HD static B other(const B& v) {
-        B r;
-#ifdef __CUDA_ARCH__
-        const unsigned pm = pmask();
-#pragma unroll
-        for (int i = 0; i < B::N; i++) r.v[i] = __shfl_xor_sync(pm, v.v[i], 1);
-#elif defined(SB_PAIR_HOST_EMULATE)
-        sb_pair_exchange(v.v, r.v, B::N);
-#else
-        r = v;
-#endif
-        return r;
-    }
-    SB_HD static bool pair_all(bool p) {
-#ifdef __CUDA_ARCH__
-        return __all_sync(pmask(), p) != 0;
-#elif defined(SB_PAIR_HOST_EMULATE)
-        return sb_pair_all(p);
-#else
-        return p;
-#endif
-    }
-    SB_HD static B sel(bool c, const B& a, const B& b) {
-        B r;
-#pragma unroll
-        for (int i = 0; i < B::N; i++) r.v[i] = c ? a.v[i] : b.v[i];
-        return r;
-    }
-    SB_HD static Fp2L zero() { Fp2L r; r.m = B::zero(); return r; }
-    SB_HD static Fp2L one() { Fp2L r; r.m = sel(odd(), B::zero(), B::one()); return r; }
-    SB_HD bool is_zero() const { return pair_all(m.is_zero()); }
-    SB_HD bool operator==(const Fp2L& o) const { return pair_all(m == o.m); }
-    SB_HD static Fp2L add(const Fp2L& x, const Fp2L& y) { Fp2L r; r.m = B::add(x.m, y.m); return r; }
-    SB_HD static Fp2L sub(const Fp2L& x, const Fp2L& y) { Fp2L r; r.m = B::sub(x.m, y.m); return r; }
-    SB_HD static Fp2L dbl(const Fp2L& x) { Fp2L r; r.m = B::dbl(x.m); return r; }
-    SB_HD static Fp2L neg(const Fp2L& x) { Fp2L r; r.m = B::neg(x.m); return r; }
-    SB_HD static Fp2L cneg(const Fp2L& x, bool f) { Fp2L r; r.m = B::cneg(x.m, f); return r; }
-    SB_HD static Fp2L mul_i(const Fp2L& x, const Fp2L& y) {
-        const bool o = odd();
-        const B xo = other(x.m), yo = other(y.m);
-        // even lane (mine = c0): x.a*y.a + x.b*(-y.b);   odd lane (mine = c1): x.b*y.a + x.a*y.b   =>   x.mine*Pv + x.other*Qv
-        const B Pv = sel(o, yo, y.m), Qv = sel(o, y.m, B::neg(yo));
-        Fp2L r; r.m = B::mul2_i(x.m, Pv, xo, Qv); return r;
-    }
-    SB_HD static Fp2L sqr_i(const Fp2L& x) {
-        const bool o = odd();
-        const B xo = other(x.m);
-        const B U = B::add(sel(o, xo, x.m), xo), V = sel(o, x.m, B::sub(x.m, xo));
-        Fp2L r; r.m = B::mul(U, V); return r;
-    }
-    SB_HD_NOINLINE static Fp2L mul(const Fp2L& x, const Fp2L& y) { return mul_i(x, y); }
-    SB_HD_NOINLINE static Fp2L sqr(const Fp2L& x) { return sqr_i(x); }
-};
-
 // Affine point (x, y); infinity = (0, 0) (reference 6068-6086).
 template <class F> struct Affine {
     F x, y;

@@ -138,59 +138,6 @@ k_accumulate(const Affine<F>* __restrict__ bases, const uint32_t* __restrict__ k
     else store_vec(buckets + cur, acc);
 }
 
-// The same walk for an extension-field group with every point spread over a lane pair (Fp2L, ec.cuh): thread 2t holds the c0
-// components of segment t's accumulator, thread 2t+1 the c1 components.  Half the registers per thread (the plain kernel needs
-// 252 and runs 8 warps per SM), twice the threads; the arithmetic per point is the same 16 dual products + 4 multiplies, split
-// evenly over the two lanes.  Memory layout is unchanged (x.c0 x.c1 y.c0 y.c1 zz.c0 ...): lane `par` moves the blocks 2k + par.
-template <class T> struct fp2_param;
-template <class P> struct fp2_param<Fp2<P>> { typedef P type; };
-template <class P, int MINB>
-__global__ void __launch_bounds__(MSM_ACC_THREADS, MINB)
-k_accumulate_pair(const Affine<Fp2<P>>* __restrict__ bases, const uint32_t* __restrict__ keys, const uint32_t* __restrict__ vals,
-                  const uint64_t* __restrict__ counts, XYZZ<Fp2<P>>* __restrict__ buckets,
-                  XYZZ<Fp2<P>>* __restrict__ heads, uint32_t* __restrict__ head_keys) {
-    typedef Fp2L<P> F; typedef Fp<P> B;
-    const uint64_t M = counts[0];
-    const uint32_t seg = (uint32_t)counts[MSM_COUNTS_SEG];
-    const uint64_t t = (blockIdx.x * (uint64_t)blockDim.x + threadIdx.x) >> 1;
-    const uint32_t par = threadIdx.x & 1u;
-    uint64_t lo = t * seg;
-    if (lo >= M) return;                                     // both lanes of a pair leave together
-    uint64_t hi = lo + seg < M ? lo + seg : M;
-    const F one = F::one();
-    XYZZ<F> acc = XYZZ<F>::inf();
-    auto put = [&](XYZZ<Fp2<P>>* dst, const XYZZ<F>& a) {
-        B* q = reinterpret_cast<B*>(dst);
-        store_vec(q + par, a.x.m); store_vec(q + 2 + par, a.y.m); store_vec(q + 4 + par, a.zz.m); store_vec(q + 6 + par, a.zzz.m);
-    };
-    uint32_t cur = keys[lo];
-    bool first = true;
-    for (uint64_t e = lo; e < hi; e++) {
-        uint32_t k = keys[e], v = vals ? vals[e] : (uint32_t)e;
-        if (k != cur) {
-            if (first) { put(heads + t, acc); if (!par) head_keys[t] = cur; first = false; }
-            else put(buckets + cur, acc);
-            acc = XYZZ<F>::inf(); cur = k;
-        }
-        F px, py;
-        {
-            constexpr int NV = sizeof(B) / 16;
-            const uint4* p = reinterpret_cast<const uint4*>(reinterpret_cast<const B*>(bases + (v & 0x7fffffffu)) + par);
-            uint4* dx = reinterpret_cast<uint4*>(&px.m); uint4* dy = reinterpret_cast<uint4*>(&py.m);
-#pragma unroll
-            for (int i = 0; i < NV; i++) dx[i] = __ldg(p + i);
-#pragma unroll
-            for (int i = 0; i < NV; i++) dy[i] = __ldg(p + 2 * NV + i);
-        }
-        if (!(px.is_zero() & py.is_zero())) {
-            py = F::cneg(py, (v >> 31) != 0);
-            acc.add_affine(px, py, one);
-        }
-    }
-    if (first) { put(heads + t, acc); if (!par) head_keys[t] = cur; }
-    else put(buckets + cur, acc);
-}
-
 // ------------------------------------------------------------------------------------------------
 // level 1 fast path: one thread per head partial.  Heads are sorted by key; a run of equal keys of length
 // <= MSM_SHORT_RUN is summed by its first thread and added to the bucket (for uniform scalars practically every
@@ -299,75 +246,6 @@ k_reduce(const XYZZ<F>* __restrict__ buckets, MsmGeom g, XYZZ<F>* __restrict__ p
         __syncthreads();
     }
     if (threadIdx.x == 0) store_vec(partials + (uint64_t)w * ctas_per_window + cta, load_vec(sm));
-}
-
-// ------------------------------------------------------------------------------------------------
-// Hierarchical bucket reduction (used when a window has >= 2048 buckets).  For a block of buckets [b0, b0+n):
-//   R = sum B_b,   S = sum (b - b0 + 1) * B_b.
-// m adjacent blocks of n buckets combine as  R = sum R_i,  S = sum S_i + n * sum_i i*R_i, where sum_i i*R_i is again a
-// running sum (t += R_i; acc += t from the top).  So every level costs ~3 additions per child and log2(n) doublings
-// per parent — no per-thread scalar multiply as in k_reduce (which spends ~40 % of its work there).
-// k_reduce2: one CTA = 128 threads x 16 buckets (level 1) -> 16 groups of 8 -> 4 groups of 4 -> 1: (R, S) of 2048 buckets.
-// k_window_sum2: one CTA per window folds the per-CTA (R, S) pairs, 8 at a time, down to the window total S.
-// ------------------------------------------------------------------------------------------------
-template <class F>
-__device__ __forceinline__ void combine_children(const XYZZ<F>* Rin, const XYZZ<F>* Sin, int m, int log_n, XYZZ<F>& Rout, XYZZ<F>& Sout) {
-    XYZZ<F> t = XYZZ<F>::inf(), acc = XYZZ<F>::inf(), ssum = load_vec(Sin);
-    for (int i = m - 1; i >= 1; i--) {
-        XYZZ<F> r = load_vec(Rin + i), s = load_vec(Sin + i);
-        t.add(r); acc.add(t); ssum.add(s);
-    }
-    for (int k = 0; k < log_n; k++) acc = XYZZ<F>::dbl(acc);
-    ssum.add(acc);
-    XYZZ<F> r0 = load_vec(Rin); t.add(r0);
-    Rout = t; Sout = ssum;
-}
-
-static constexpr int RED2_L = 16, RED2_THREADS = 128, RED2_BUCKETS = RED2_L * RED2_THREADS;   // 2048 buckets per CTA
-
-template <class F>
-__global__ void __launch_bounds__(RED2_THREADS)
-k_reduce2(const XYZZ<F>* __restrict__ buckets, MsmGeom g, XYZZ<F>* __restrict__ outR, XYZZ<F>* __restrict__ outS) {
-    extern __shared__ uint4 smem_raw[];
-    XYZZ<F>* sm = reinterpret_cast<XYZZ<F>*>(smem_raw);
-    XYZZ<F>* R1 = sm; XYZZ<F>* S1 = sm + 128; XYZZ<F>* R2 = sm + 256; XYZZ<F>* S2 = sm + 272; XYZZ<F>* R3 = sm + 288; XYZZ<F>* S3 = sm + 292;
-    const uint32_t tid = threadIdx.x;
-    const XYZZ<F>* bk = buckets + (uint64_t)blockIdx.x * RED2_BUCKETS + (uint64_t)tid * RED2_L;
-    {   // level 1: classic running sum over 16 buckets
-        XYZZ<F> run = XYZZ<F>::inf(), sum = XYZZ<F>::inf();
-        for (int b = RED2_L - 1; b >= 0; b--) { XYZZ<F> p = load_vec(bk + b); run.add(p); sum.add(run); }
-        store_vec(R1 + tid, run); store_vec(S1 + tid, sum);
-    }
-    __syncthreads();
-    if (tid < 16) { XYZZ<F> r, s; combine_children<F>(R1 + 8 * tid, S1 + 8 * tid, 8, 4, r, s); store_vec(R2 + tid, r); store_vec(S2 + tid, s); }   // n = 16
-    __syncthreads();
-    if (tid < 4) { XYZZ<F> r, s; combine_children<F>(R2 + 4 * tid, S2 + 4 * tid, 4, 7, r, s); store_vec(R3 + tid, r); store_vec(S3 + tid, s); }      // n = 128
-    __syncthreads();
-    if (tid == 0) { XYZZ<F> r, s; combine_children<F>(R3, S3, 4, 9, r, s); store_vec(outR + blockIdx.x, r); store_vec(outS + blockIdx.x, s); }      // n = 512
-}
-
-// per window: NC = B / 2048 pairs (power of two, <= 1024) -> S of the window.  One CTA of 128 threads per window.
-template <class F>
-__global__ void __launch_bounds__(128)
-k_window_sum2(const XYZZ<F>* __restrict__ inR, const XYZZ<F>* __restrict__ inS, uint32_t NC, XYZZ<F>* __restrict__ out) {
-    extern __shared__ uint4 smem_raw[];
-    XYZZ<F>* sm = reinterpret_cast<XYZZ<F>*>(smem_raw);     // two ping-pong regions of (R[128], S[128])
-    const uint32_t tid = threadIdx.x;
-    const XYZZ<F>* Rin = inR + (uint64_t)blockIdx.x * NC; const XYZZ<F>* Sin = inS + (uint64_t)blockIdx.x * NC;
-    uint32_t n = NC; int log_block = 11;                    // a child covers 2^11 buckets at the first level
-    int ping = 0;
-    while (n > 1) {
-        const uint32_t m = n >= 8 ? 8 : n, parents = n / m;
-        XYZZ<F>* Rout = sm + ping * 256; XYZZ<F>* Sout = Rout + 128;
-        for (uint32_t p = tid; p < parents; p += blockDim.x) {
-            XYZZ<F> r, s; combine_children<F>(Rin + (uint64_t)p * m, Sin + (uint64_t)p * m, (int)m, log_block, r, s);
-            store_vec(Rout + p, r); store_vec(Sout + p, s);
-        }
-        __syncthreads();
-        Rin = Rout; Sin = Sout; n = parents; ping ^= 1;
-        log_block += (m == 8 ? 3 : m == 4 ? 2 : 1);
-    }
-    if (tid == 0) store_vec(out + blockIdx.x, load_vec(Sin));
 }
 
 // one warp per window: lanes stride over the per-CTA partials of k_reduce, then a shared-memory tree
@@ -603,10 +481,6 @@ __global__ void __launch_bounds__(128) k_gen_points(Affine<F> g, uint64_t seed, 
     store_vec(out + i, a);
 }
 
-}  // namespace sb
-#include "msm_pair.cuh"
-namespace sb {
-
 // ------------------------------------------------------------------------------------------------
 // Device scratch (grow-only) and the two halves of the pipeline.
 // ------------------------------------------------------------------------------------------------
@@ -619,7 +493,8 @@ struct MsmScratch {
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
 
-extern int g_msm_tuning[12];
+// sb_set_tuning(1, 1): reduce the buckets with k_reduce / k_window_sum even where ws_plan accepts the geometry
+extern int g_msm_force_reduce;
 
 struct MsmLaunchStats {
     int launches = 0;
@@ -653,12 +528,6 @@ struct MsmSorted {
     uint32_t seg_lo = MSM_SEG;
 };
 
-// msm_sort.cu: helpers of the pairing rounds (non-template part)
-size_t msm_pair_scan_tmp_bytes(uint32_t NB);
-int msm_pair_offsets(const uint32_t* keys, const uint64_t* counts, uint32_t NB, uint32_t* off, cudaStream_t stream);
-int msm_pair_next_offsets(const uint32_t* off_in, uint32_t NB, uint32_t* sizes, uint32_t* off_out, void* tmp, size_t tmp_bytes, cudaStream_t stream);
-int msm_pair_counts(const uint32_t* off, uint32_t NB, uint64_t* counts, cudaStream_t stream);
-
 // msm_sort.cu: digits + radix sort + valid count.  d_scalars is a device pointer.
 int msm_sort_entries(const uint8_t* d_scalars, uint32_t sbytes, uint64_t n, MsmGeom g, MsmScratch& scratch,
                      cudaStream_t stream, MsmSorted* out, MsmLaunchStats* stats);
@@ -668,83 +537,8 @@ int msm_sort_entries(const uint8_t* d_scalars, uint32_t sbytes, uint64_t n, MsmG
 // (fold, bucket reduction, window sum) on `tail_stream` after `ev_acc` (recorded here): with a higher-priority tail
 // stream the tail of one MSM slips into the SM slots freed by the next MSM's accumulation instead of queueing behind it.
 template <class F>
-int msm_buckets_impl(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& scratch, size_t scratch_off, cudaStream_t stream,
-                     XYZZ<F>* d_wsum, MsmLaunchStats* stats, cudaStream_t tail_stream, cudaEvent_t ev_acc);
-
-// Entry: optional batched-affine pairing rounds (msm_pair.cuh) shrink the entry list first, then the segmented XYZZ
-// pipeline runs on what is left.  EXPERIMENTAL, off by default (enable with sb_set_tuning(4, 2), cap the rounds with
-// sb_set_tuning(5, R)): the rounds (scan + shared inversion + two gather passes) keep the integer pipe less busy than
-// the XYZZ accumulation does, which cancels their 6-vs-10 modmul advantage.
-template <class F>
 int msm_buckets(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& scratch, cudaStream_t stream,
                 XYZZ<F>* d_wsum, MsmLaunchStats* stats, cudaStream_t tail_stream = nullptr, cudaEvent_t ev_acc = nullptr) {
-    const MsmGeom g = s.g;
-    const uint64_t NBl = (uint64_t)g.windows() * g.B;
-    const double avg = NBl ? (double)s.total / (double)NBl : 0.0;
-    if (g_msm_tuning[4] != 2 || avg < 4.0 || NBl >= (1ull << 31) || s.total >= (1ull << 31))
-        return msm_buckets_impl<F>(d_bases, s, scratch, 0, stream, d_wsum, stats, tail_stream, ev_acc);
-    const uint32_t NB = (uint32_t)NBl;
-    int R = 1; while ((1u << R) < 2.0 * avg && R < 8) R++;
-    if (g_msm_tuning[5] > 0 && g_msm_tuning[5] < R) R = g_msm_tuning[5];   // cap on the number of pairing rounds (experiments)
-    auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-    const uint64_t ub1 = (s.total + NB + 1) / 2;
-    const size_t scan_tmp = msm_pair_scan_tmp_bytes(NB);
-    const uint64_t pthreads = ((ub1 + PAIR_K - 1) / PAIR_K + PAIR_THREADS - 1) / PAIR_THREADS * PAIR_THREADS;
-    size_t o_offA = 0, o_offB = o_offA + al((size_t)(NB + 1) * 4), o_sizes = o_offB + al((size_t)(NB + 1) * 4);
-    size_t o_tmp = o_sizes + al((size_t)(NB + 1) * 4), o_cnt = o_tmp + al(scan_tmp);
-    size_t o_PA = o_cnt + 256, o_PB = o_PA + al(ub1 * sizeof(Affine<F>)), o_KA = o_PB + al(ub1 * sizeof(Affine<F>));
-    size_t o_KB = o_KA + al(ub1 * 4), o_L = o_KB + al(ub1 * 4), o_rest = o_L + al(pthreads * PAIR_K * sizeof(F));
-    // size the rest (buckets, heads, partials) for the list that survives the rounds
-    uint64_t ub = s.total; for (int r = 0; r < R; r++) ub = (ub + NB + 1) / 2;
-    MsmSorted s2 = s; s2.total = ub; s2.vals = nullptr; s2.seg_lo = MSM_SEG;
-    // first call sizes the whole scratch: probe the tail's requirement with a dry computation (same formula as impl)
-    {
-        const uint64_t heads0 = (ub + MSM_SEG - 1) / MSM_SEG, heads1 = (heads0 + MSM_SEG - 1) / MSM_SEG;
-        const uint32_t L = g.B < (uint32_t)MSM_RED_CHUNK ? g.B : MSM_RED_CHUNK;
-        const uint32_t ctas_per_window = (g.B / L + 127) / 128;
-        size_t need = al(NBl * sizeof(XYZZ<F>)) + al(heads0 * sizeof(XYZZ<F>)) + al(heads0 * 4) + al(heads1 * sizeof(XYZZ<F>)) + al(heads1 * 4) +
-                      al(heads0 * 4) + al(msm_reduce_scratch_elems(g) * sizeof(XYZZ<F>));
-        need += need / 8 + (1u << 20);   // margin: the impl must never grow (= reallocate) the scratch the rounds are using
-        if (!scratch.get(o_rest + need)) return (int)cudaErrorMemoryAllocation;
-    }
-    uint8_t* base = (uint8_t*)scratch.p;
-    uint32_t* offA = (uint32_t*)(base + o_offA); uint32_t* offB = (uint32_t*)(base + o_offB); uint32_t* sizes = (uint32_t*)(base + o_sizes);
-    uint64_t* counts2 = (uint64_t*)(base + o_cnt);
-    Affine<F>* P[2] = {(Affine<F>*)(base + o_PA), (Affine<F>*)(base + o_PB)};
-    uint32_t* K[2] = {(uint32_t*)(base + o_KA), (uint32_t*)(base + o_KB)};
-    F* Ls = (F*)(base + o_L);
-    int launches = 0;
-    ProfScope prof(stats, stats ? stats->cur_tag : 0, stream);
-    int rc = msm_pair_offsets(s.keys, s.counts, NB, offA, stream); launches++;
-    if (rc) return rc;
-    const Affine<F>* src = d_bases; uint32_t* in = offA; uint32_t* out = offB;
-    uint64_t ubr = s.total;
-    for (int r = 0; r < R; r++) {
-        rc = msm_pair_next_offsets(in, NB, sizes, out, base + o_tmp, scan_tmp, stream); launches += 3;
-        if (rc) return rc;
-        ubr = (ubr + NB + 1) / 2;
-        const unsigned grid = (unsigned)(((ubr + PAIR_K - 1) / PAIR_K + PAIR_THREADS - 1) / PAIR_THREADS);
-        if (r == 0) k_pair_round<F, true><<<grid, PAIR_THREADS, 0, stream>>>(src, s.vals, in, out, NB, P[0], K[0], Ls);
-        else k_pair_round<F, false><<<grid, PAIR_THREADS, 0, stream>>>(src, nullptr, in, out, NB, P[r & 1], K[r & 1], Ls);
-        launches++;
-        src = P[r & 1]; s2.keys = K[r & 1];
-        uint32_t* t = in; in = out; out = t;
-    }
-    rc = msm_pair_counts(in, NB, counts2, stream); launches++;
-    if (rc) return rc;
-    s2.counts = counts2;
-    prof.end();
-    if (stats) stats->launches += launches;
-    // the segmented pipeline on the reduced list; its own accumulate launch is not separately profiled (nev guard)
-    cudaEvent_t* sev = stats ? stats->ev : nullptr; if (stats) stats->ev = nullptr;
-    rc = msm_buckets_impl<F>(src, s2, scratch, o_rest, stream, d_wsum, stats, tail_stream, ev_acc);
-    if (stats) stats->ev = sev;
-    return rc;
-}
-
-template <class F>
-int msm_buckets_impl(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& scratch, size_t scratch_off, cudaStream_t stream,
-                     XYZZ<F>* d_wsum, MsmLaunchStats* stats, cudaStream_t tail_stream, cudaEvent_t ev_acc) {
     const MsmGeom g = s.g;
     const uint32_t NW = g.windows();
     const uint64_t nbuckets = (uint64_t)NW * g.B;
@@ -761,9 +555,8 @@ int msm_buckets_impl(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& s
     size_t o_hkM = o_hkB + al(heads1 * 4);                     // level-1 keys after the short-run fast path
     size_t o_part = o_hkM + al(heads0 * 4);
     size_t bytes = o_part + al(msm_reduce_scratch_elems(g) * sizeof(XYZZ<F>));
-    uint8_t* base = (uint8_t*)scratch.get(scratch_off + bytes);
+    uint8_t* base = (uint8_t*)scratch.get(bytes);
     if (!base) return (int)cudaErrorMemoryAllocation;
-    base += scratch_off;
     XYZZ<F>* buckets = (XYZZ<F>*)(base + o_buckets);
     XYZZ<F>* headsA = (XYZZ<F>*)(base + o_headsA); uint32_t* hkA = (uint32_t*)(base + o_hkA);
     XYZZ<F>* headsB = (XYZZ<F>*)(base + o_headsB); uint32_t* hkB = (uint32_t*)(base + o_hkB);
@@ -775,38 +568,14 @@ int msm_buckets_impl(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& s
         ProfScope prof(stats, stats ? stats->cur_tag : 0, stream);
         {
             const unsigned grid = (unsigned)((heads0 + MSM_ACC_THREADS - 1) / MSM_ACC_THREADS);
-            // occupancy variants (sb_set_tuning(0, minBlocksPerSM)): base-field groups run best at 4 CTAs/SM (124 regs);
-            // extension-field groups (accumulator = 64-96 registers) have their own variants
-            constexpr bool ext = sizeof(F) > 48 && (sizeof(F) % 64 == 0 || sizeof(F) == 96);
-            if constexpr (ext) {
-                typedef typename fp2_param<F>::type FP;
-                const unsigned pgrid = (unsigned)((2 * heads0 + MSM_ACC_THREADS - 1) / MSM_ACC_THREADS);
-                if (g_msm_tuning[9] == 4) k_accumulate_pair<FP, 4><<<pgrid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA);
-                else if (g_msm_tuning[9] == 3) k_accumulate_pair<FP, 3><<<pgrid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA);
-                else switch (g_msm_tuning[0]) {
-                case 3: k_accumulate<F, 3><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;
-                case 4: k_accumulate<F, 4><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;
-                default: k_accumulate<F, 2><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;   // H100 (400 W), 2^20 G2: 7.6 ms vs 8.3 (3), 9.2 (4), 8.3 (lane pair)
-                }
-            } else if constexpr (sizeof(F) > 32) {
-                // 12-limb base field (BLS12-381 G1).  At 4 CTAs/SM the 128-register cap spills ~50 words of the mixed addition
-                // (ptxas, sm_90a: 184 B spill stores / 132 B loads); 3 CTAs/SM (167 registers) and 2 (182) do not spill.  Measured on an
-                // H100 at 400 W (PLONK BLS12-381 2^18, nine accumulations): 2 CTAs/SM 15.5 ms, 4 CTAs/SM 16.7 ms, 3 CTAs/SM 19.1 ms
-                // -> 2 is the default; sb_set_tuning(10, 3 | 4) selects the others.
-                switch (g_msm_tuning[8]) {
-                case 4: k_accumulate<F, 4><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;
-                case 3: k_accumulate<F, 3><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;
-                default: k_accumulate<F, 2><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;
-                }
-            } else {
-                // 8-limb base field (BN254 G1): 116 registers at 4 CTAs/SM, no spills; sb_set_tuning(12, 3 | 2) = lower-occupancy
-                // builds (H100 at 400 W, 2^20 Groth16: all three within 1 %)
-                switch (g_msm_tuning[10]) {
-                case 3: k_accumulate<F, 3><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;
-                case 2: k_accumulate<F, 2><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;
-                default: k_accumulate<F, 4><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA); break;
-                }
-            }
+            // minBlocksPerSM per coordinate field, measured on an H100 at 400 W:
+            // - extension field (G2): 2.  2^20 G2 accumulation 7.6 ms, vs 8.3 at 3 and 9.2 at 4.
+            // - 12-limb base field (BLS12-381 G1): 2.  At 4 the 128-register cap spills ~50 words of the mixed addition (ptxas,
+            //   sm_90a: 184 B spill stores / 132 B loads); 3 (167 registers) and 2 (182) do not spill.  Nine accumulations of a
+            //   2^18 PLONK BLS12-381 proof: 15.5 ms at 2, 16.7 at 4, 19.1 at 3.
+            // - 8-limb base field (BN254 G1): 4 (116 registers, no spills).  2^20 Groth16: 2, 3 and 4 within 1 %.
+            constexpr int MINB = sizeof(F) > 32 ? 2 : 4;
+            k_accumulate<F, MINB><<<grid, MSM_ACC_THREADS, 0, stream>>>(d_bases, s.keys, s.vals, s.counts, buckets, headsA, hkA);
             launches++;
         }
         prof.end();
@@ -833,7 +602,7 @@ int msm_buckets_impl(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& s
     if (!heads0 && tail_stream && tail_stream != stream && ev_acc) { cudaEventRecord(ev_acc, stream); cudaStreamWaitEvent(tail_stream, ev_acc, 0); stream = tail_stream; }
     ProfScope pred(stats, PROF_REDUCE, stream);
     const WsPlan wp = ws_plan(g);
-    if (wp.ok && g_msm_tuning[1] == 0) {
+    if (wp.ok && !g_msm_force_reduce) {
         // axis sums (rows and columns of one level per launch), then the warp-shuffle weighted sums
         XYZZ<F>* rowb[2] = {partials, partials + wp.rowA};
         XYZZ<F>* colb[2] = {partials + wp.rowA + wp.rowB, partials + wp.rowA + wp.rowB + wp.colA};
@@ -852,19 +621,6 @@ int msm_buckets_impl(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& s
         const uint32_t per = wp.nR + wp.nC;
         k_ws_chunks<F><<<(NW * per + 3) / 4, 128, 0, stream>>>(wp.lenR ? rin : nullptr, wp.lenR, cin, wp.lenC, NW, tw); launches++;
         k_ws_final<F><<<NW, 128, 0, stream>>>(tw, wp.nR, wp.nC, d_wsum); launches++;
-    } else if (g.B >= (uint32_t)RED2_BUCKETS && g.B / RED2_BUCKETS <= 1024 && g_msm_tuning[1] == 2) {   // experimental: less work (-36 %) but 2-3x the
-        // dependent-add latency of k_reduce; measured slower (proof 27.4 ms vs 26.0 ms overlapped, 31.3 vs 26.6 serialised)
-        // hierarchical reduction: per-CTA (R, S) pairs live in the partials area (2 * NC entries per window <= ctas_per_window)
-        const uint32_t NC = g.B / RED2_BUCKETS;
-        XYZZ<F>* pR = partials; XYZZ<F>* pS = partials + (size_t)NW * NC;
-        static bool configured = false;
-        if (!configured) {
-            cudaFuncSetAttribute(k_reduce2<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(296 * sizeof(XYZZ<F>)));
-            cudaFuncSetAttribute(k_window_sum2<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(512 * sizeof(XYZZ<F>)));
-            configured = true;
-        }
-        k_reduce2<F><<<NW * NC, RED2_THREADS, 296 * sizeof(XYZZ<F>), stream>>>(buckets, g, pR, pS); launches++;
-        k_window_sum2<F><<<NW, 128, 512 * sizeof(XYZZ<F>), stream>>>(pR, pS, NC, d_wsum); launches++;
     } else {
         k_reduce<F><<<NW * ctas_per_window, red_threads, red_threads * sizeof(XYZZ<F>), stream>>>(buckets, g, partials, ctas_per_window); launches++;
         k_window_sum<F><<<NW, 32, 32 * sizeof(XYZZ<F>), stream>>>(partials, ctas_per_window, d_wsum); launches++;

@@ -421,7 +421,9 @@ def test_bigbuffer_like_inputs(bn):
 
 
 def test_msm_plain_vs_table_mode(bn):
-    """Registered bases use precomputed window tables; sb_set_tuning(3,1) forces the plain windowed path — same bytes."""
+    """Registered bases use precomputed window tables; sb_set_tuning(3,1) forces the plain windowed path — same bytes.
+    sb_set_tuning(1,1) replaces the axis-sum bucket reduction by k_reduce / k_window_sum (the path for geometries with
+    more than 2^20 buckets per window) — same bytes again, in both modes."""
     n = 1 << 14
     bases = O.gen_points(BN, 2, 21, n)
     sc = rand_fr(22, n)
@@ -431,6 +433,13 @@ def test_msm_plain_vs_table_mode(bn):
     try:
         h2 = bn.G2.registerBases(bases)
         b = bn.G2.multiExpRegistered(h2, sc)
+        assert bn.lib.sb_set_tuning(1, 2) != 0 and bn.lib.sb_set_tuning(4, 2) != 0   # unknown values and keys are refused
+        assert bn.lib.sb_set_tuning(1, 1) == 0
+        try:
+            assert bn.G2.multiExpRegistered(h2, sc).tobytes() == a.tobytes()
+            assert bn.G2.multiExpRegistered(h1, sc).tobytes() == a.tobytes()
+        finally:
+            bn.lib.sb_set_tuning(1, 0)
     finally:
         bn.lib.sb_set_tuning(3, 0)
     assert a.tobytes() == b.tobytes()
@@ -460,32 +469,6 @@ def test_groth16_sharded_keys_match_unsharded(bn):
         keys[0].prove_raw(w, r, s)
     for k in keys + [full]:
         k.release()
-
-
-def test_msm_pairing_rounds_experimental(bn):
-    """The batched-affine pairing rounds (msm_pair.cuh, off by default) give the same bytes, including the special cases
-    inside a pair: infinity operands, P + P, P + (-P)."""
-    n = 1 << 13
-    bases = O.gen_points(BN, 1, 31, n).reshape(n, 64).copy()
-    sc = rand_fr(32, n).reshape(n, 32).copy()
-    bases[3] = 0; bases[4] = 0
-    bases[500:540] = bases[500]; sc[500:540] = sc[500]           # equal points with equal scalars: doublings in every round
-    ci = O.CURVES[BN]
-    bases[601, :32] = bases[600, :32]
-    bases[601, 32:] = np.frombuffer(ci.fq_to_mont((ci.q - ci.fq_from_mont(bases[600, 32:].tobytes())) % ci.q), np.uint8)
-    sc[601] = sc[600]                                             # P and -P in the same bucket
-    want1 = O.g_to_affine(BN, 1, O.multiexp_affine(BN, 1, bases.reshape(-1), sc.reshape(-1)))
-    b2 = O.gen_points(BN, 2, 33, n)
-    want2 = O.g_to_affine(BN, 2, O.multiexp_affine(BN, 2, b2, sc.reshape(-1)))
-    bn.lib.sb_set_tuning(4, 2)
-    try:
-        for cap in (0, 2):
-            bn.lib.sb_set_tuning(5, cap)
-            assert bn.G1.toAffine(bn.G1.multiExpAffine(bases.reshape(-1), sc.reshape(-1))).tobytes() == want1
-            h = bn.G2.registerBases(b2)
-            assert bn.G2.toAffine(bn.G2.multiExpRegistered(h, sc.reshape(-1))).tobytes() == want2
-    finally:
-        bn.lib.sb_set_tuning(4, 0); bn.lib.sb_set_tuning(5, 0)
 
 
 def test_plonk_polynomial_wrappers_on_fixture_goldens(bn, golden):

@@ -19,18 +19,6 @@ def test_host_fp_check(tmp_path, flags):
     assert out.returncode == 0 and "HOST CHECK PASSED" in out.stdout, out.stdout + out.stderr
 
 
-@pytest.mark.parametrize("flags", [["-DSB_HOST_EMULATE_PTX"], []])
-def test_host_lane_pair_check(tmp_path, flags):
-    """Fp2L (ec.cuh): the lane-pair form of Fq2 that k_accumulate_pair runs, two host threads in lockstep as the two lanes,
-    against the plain Fp2 / XYZZ<Fp2> code on both curves (multiplies, squarings, votes, mixed additions incl. doubling,
-    cancellation, y = 0 and infinity)."""
-    exe = str(tmp_path / "host_pair_check")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-pthread", "-DSB_PAIR_HOST_EMULATE", *flags, "-o", exe,
-                           os.path.join(ROOT, "tests", "host", "host_pair_check.cpp")])
-    out = subprocess.run([exe], capture_output=True, text=True, timeout=600)
-    assert out.returncode == 0 and "PAIR CHECK PASSED" in out.stdout, out.stdout + out.stderr
-
-
 def test_zkey_parsers_survive_mutation_fuzzing(tmp_path, golden):
     """plonk_parse_zkey / fflonk_parse_zkey (the code sb_plonk_load / sb_fflonk_load run on caller bytes) and the host-side
     load logic behind them, under AddressSanitizer + UBSan on mutated containers: truncations, bit flips in the section
