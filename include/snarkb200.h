@@ -208,6 +208,10 @@ double sb_calibrate(sb_ctx* ctx, int what);
  *   6  log2 of the points per MSM chunk (test hook; 0 = default)
  *   7  log2 of the largest NTT tile (10..12)
  *   8  0 = no pinned staging of pageable host buffers
+ *  13  MSM window bits c, 3..22 (test hook; 0 = default: chosen from the number of points).  Applies wherever a geometry
+ *      is chosen: per chunk for MSMs on unregistered bases, and for window tables when they are built, i.e. when bases are
+ *      registered or a key is loaded; a table keeps the c in force at that moment.  Tables are still skipped when
+ *      W * n >= 2^31.  A large c costs memory: a plain MSM allocates W * 2^(c-1) buckets.
  * The Python mirror applies SB_TUNE="key=value,..." from the environment when it loads the library. */
 int sb_set_tuning(int key, int value);
 /* synthetic bases for tests/benchmarks: chunks of 4096 points P_{c,j} = (k0(seed, c) + j*kd(seed)) * G, affine Montgomery, computed

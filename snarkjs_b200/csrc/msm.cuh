@@ -30,6 +30,9 @@ static constexpr int MSM_RED_CHUNK = 16;    // buckets per thread in k_reduce
 static constexpr uint32_t MSM_INVALID_KEY = 0xffffffffu;
 static constexpr int MSM_COUNTS_SEG = 8;      // counts[8]: sorted entries per k_accumulate thread (counts[0] = valid entries, [1..7] = fold level sizes)
 
+// sb_set_tuning(13, c): window bits (3..22) that msm_choose and msm_geometry_precomp return instead of their own choice
+// (test hook; 0 = the heuristics below)
+extern int g_msm_force_c;
 
 // Window-size choice.  Cost model: W_eff*n mixed adds (10 modmul) + one pass over the buckets (~60 modmul each);
 // buckets = 2^(c-1) per window, shared by all windows in the precomputed-table mode.  `fr_bits` is the bit length of
@@ -48,6 +51,7 @@ __host__ inline MsmGeom msm_choose(uint64_t n, uint32_t scalar_bytes, int fr_bit
         double cost = (double)weff * (double)n * 10.0 + buckets * 60.0;
         if (cost < best) { best = cost; best_c = c; }
     }
+    if (g_msm_force_c) best_c = g_msm_force_c;
     MsmGeom g; g.c = best_c; g.W = (int)((8 * scalar_bytes + 1 + best_c - 1) / best_c); g.B = 1u << (best_c - 1);
     return g;
 }
@@ -64,6 +68,7 @@ __host__ inline MsmGeom msm_geometry_precomp(uint64_t n_set, uint32_t scalar_byt
         if (weff > 1 && top < cc - 5) continue;
         c = cc; break;
     }
+    if (g_msm_force_c) c = g_msm_force_c;
     MsmGeom g; g.c = c; g.W = (int)((8 * scalar_bytes + 1 + c - 1) / c); g.B = 1u << (c - 1);
     g.precomp = 1; g.stride = n_set; g.first = 0;
     return g;

@@ -5,6 +5,7 @@
 namespace sb {
 
 int g_msm_force_reduce = 0;
+int g_msm_force_c = 0;
 
 // ------------------------------------------------------------------------------------------------
 // digits: thread i recodes scalar i into W signed digits (reference _getChunk extracts unsigned chunks;

@@ -434,6 +434,7 @@ def test_msm_plain_vs_table_mode(bn):
         h2 = bn.G2.registerBases(bases)
         b = bn.G2.multiExpRegistered(h2, sc)
         assert bn.lib.sb_set_tuning(1, 2) != 0 and bn.lib.sb_set_tuning(4, 2) != 0   # unknown values and keys are refused
+        assert all(bn.lib.sb_set_tuning(13, v) != 0 for v in (1, 2, 23))           # window bits outside 3..22
         assert bn.lib.sb_set_tuning(1, 1) == 0
         try:
             assert bn.G2.multiExpRegistered(h2, sc).tobytes() == a.tobytes()
