@@ -78,6 +78,18 @@ int sb_qap_join_abc(sb_ctx* ctx, const uint8_t* a, const uint8_t* b, const uint8
 /* Fr constants the JS side reads from the curve object: what = -1 -> Fr.shift (nqr^2), -2 -> Fr.nqr,
  * 0..s -> Fr.w[what] (12866-12889).  Returns s. */
 int sb_fr_root(sb_ctx* ctx, int what, uint8_t out[32]);
+/* G1/G2.fft and G1/G2.ifft (15101-15107 -> _fft 14675-14918): n points in natural order, affine (in_jacobian = 0, infinity =
+ * all-zero bytes) or Jacobian (Z = 0 is infinity); out as affine or as Jacobian normalised to Z = 1 (infinity (0,1,0)),
+ * the MSM output convention.  inverse != 0 gives x[k] = n^-1 X[(n-k) mod n].  n must be a power of two ("fft must be
+ * multiple of 2") with log2(n) <= Fr.s; the reference's fftExt path (log2(n) = Fr.s + 1) is refused with SB_ERR_ARG.
+ * Every butterfly is one variable-base scalar multiplication on the GPU.  sb_last_ms: 0 total, 1 upload, 2 compute,
+ * 3 download.  G.lagrangeEvaluations (15109-15176) is the inverse transform for log2(n) <= Fr.s. */
+int sb_group_fft(sb_ctx* ctx, int group, const uint8_t* in, int in_jacobian, uint64_t n, int inverse,
+                 int out_jacobian, uint8_t* out);
+/* G1/G2.batchApplyKey (14268-14385): out[i] = in[i] * first * inc^i (first, inc Montgomery Fr); same point formats as
+ * sb_group_fft; n = 0 writes nothing. */
+int sb_group_batch_apply_key(sb_ctx* ctx, int group, const uint8_t* in, int in_jacobian, uint64_t n,
+                             const uint8_t first[32], const uint8_t inc[32], int out_jacobian, uint8_t* out);
 
 /* Fused Groth16 prover (src/groth16_prove.js:28-144) with every intermediate resident in HBM.
  * sb_groth16_load parses a Groth16 .zkey image (src/zkey_utils.js:229-259 + sections 4-9), uploads the five base

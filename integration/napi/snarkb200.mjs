@@ -21,6 +21,30 @@ export async function useB200(curveName = "bn128", device = 0) {
     };
   }
   const Fr = curve.Fr;
+  // G.fft / G.ifft / G.lagrangeEvaluations / G.batchApplyKey (build/snarkjs.js:15101-15176, 14268-14385): every butterfly is a
+  // scalar multiplication on the GPU.  Array inputs (one Uint8Array per point) come back as arrays, like Fr.fft below.
+  for (const [G, gid] of [[curve.G1, 1], [curve.G2, 2]]) {
+    const size = (t) => G.F.n8 * ((t || "affine") == "jacobian" ? 3 : 2);
+    const gfft = (inverse) => async (buff, inType, outType) => {
+      const isArray = Array.isArray(buff);
+      const b = isArray ? Buffer.concat(buff) : flatten(buff);
+      const n = b.byteLength / size(inType);
+      if (!Number.isInteger(Math.log2(n))) throw new Error("fft must be multiple of 2");
+      const out = new Uint8Array(await addon.groupFft(ctx, gid, b, +(inType == "jacobian"), inverse, +(outType == "jacobian"), n8q));
+      const so = size(outType);
+      return isArray ? Array.from({ length: n }, (_, i) => out.slice(i * so, (i + 1) * so)) : out;
+    };
+    G.fft = gfft(0);
+    G.ifft = gfft(1);
+    G.lagrangeEvaluations = async (buff, inType, outType) => {
+      const b = flatten(buff), bits = Math.log2(b.byteLength / size(inType));
+      if (!Number.isInteger(bits)) throw new Error("lagrangeEvaluations invalid Input size");
+      if (bits > Fr.s + 1) throw new Error("lagrangeEvaluations input too big");
+      return G.ifft(b, inType, outType);                                                     // Fr.s + 1 is refused by the library
+    };
+    G.batchApplyKey = async (buff, first, inc, inType, outType) =>
+      new Uint8Array(await addon.groupApplyKey(ctx, gid, flatten(buff), Fr.e(first), Fr.e(inc), +(inType == "jacobian"), +(outType == "jacobian"), n8q));
+  }
   const fft = (inverse) => async (buff) => {
     const isArray = Array.isArray(buff);
     const b = isArray ? Buffer.concat(buff) : flatten(buff);

@@ -95,6 +95,29 @@ Napi::Value QapJoinAbc(const Napi::CallbackInfo& info) {
   return Queue(info.Env(), c, a.ByteLength(), [=](std::vector<uint8_t>& out) { return sb_qap_join_abc(c, pa, pb, pc, n, out.data()); }, {a, b, cc});
 }
 
+// groupFft(ctx, group, buff, inJacobian, inverse, outJacobian, n8q) -> Promise<Buffer>     (G.fft / G.ifft 15101-15107)
+Napi::Value GroupFft(const Napi::CallbackInfo& info) {
+  sb_ctx* c = ctx_of(info[0]); int group = info[1].As<Napi::Number>().Int32Value(); auto buff = info[2].As<Napi::Uint8Array>();
+  int in_jac = info[3].As<Napi::Number>().Int32Value(), inverse = info[4].As<Napi::Number>().Int32Value(), out_jac = info[5].As<Napi::Number>().Int32Value();
+  size_t n8 = info[6].As<Napi::Number>().Uint32Value() * group;
+  size_t n = buff.ByteLength() / ((in_jac ? 3 : 2) * n8); const uint8_t* p = buff.Data();
+  return Queue(info.Env(), c, n * (out_jac ? 3 : 2) * n8, [=](std::vector<uint8_t>& out) {
+    return sb_group_fft(c, group, p, in_jac, n, inverse, out_jac, out.data());
+  }, {buff});
+}
+
+// groupApplyKey(ctx, group, buff, first, inc, inJacobian, outJacobian, n8q) -> Promise<Buffer>   (G.batchApplyKey 14268-14385)
+Napi::Value GroupApplyKey(const Napi::CallbackInfo& info) {
+  sb_ctx* c = ctx_of(info[0]); int group = info[1].As<Napi::Number>().Int32Value(); auto buff = info[2].As<Napi::Uint8Array>();
+  auto first = info[3].As<Napi::Uint8Array>(); auto inc = info[4].As<Napi::Uint8Array>();
+  int in_jac = info[5].As<Napi::Number>().Int32Value(), out_jac = info[6].As<Napi::Number>().Int32Value();
+  size_t n8 = info[7].As<Napi::Number>().Uint32Value() * group;
+  size_t n = buff.ByteLength() / ((in_jac ? 3 : 2) * n8); const uint8_t *p = buff.Data(), *pf = first.Data(), *pi = inc.Data();
+  return Queue(info.Env(), c, n * (out_jac ? 3 : 2) * n8, [=](std::vector<uint8_t>& out) {
+    return sb_group_batch_apply_key(c, group, p, in_jac, n, pf, pi, out_jac, out.data());
+  }, {buff, first, inc});
+}
+
 // groth16Load(ctx, zkeyBytes) -> handle (sync: done once per key) ; groth16Prove(ctx, handle, witnessSection, r, s) -> Promise<Buffer(8*n8q)>
 Napi::Value Groth16Load(const Napi::CallbackInfo& info) {
   sb_ctx* c = ctx_of(info[0]); auto z = info[1].As<Napi::Uint8Array>(); uint64_t h = 0;
@@ -158,6 +181,8 @@ Napi::Object Init(Napi::Env env, Napi::Object exports) {
   exports.Set("frBatchApplyKey", Napi::Function::New(env, FrBatchApplyKey));
   exports.Set("frConvert", Napi::Function::New(env, FrConvert));
   exports.Set("qapJoinAbc", Napi::Function::New(env, QapJoinAbc));
+  exports.Set("groupFft", Napi::Function::New(env, GroupFft));
+  exports.Set("groupApplyKey", Napi::Function::New(env, GroupApplyKey));
   exports.Set("groth16Load", Napi::Function::New(env, Groth16Load));
   exports.Set("groth16Prove", Napi::Function::New(env, Groth16Prove));
   exports.Set("groth16LoadFile", Napi::Function::New(env, Groth16LoadFile));

@@ -39,6 +39,8 @@ _SIGNATURES = {
     "sb_fr_batch_from_montgomery": (ctypes.c_int, [vp, vp, u64, vp]),
     "sb_qap_join_abc": (ctypes.c_int, [vp, vp, vp, vp, u64, vp]),
     "sb_fr_root": (ctypes.c_int, [vp, ctypes.c_int, vp]),
+    "sb_group_fft": (ctypes.c_int, [vp, ctypes.c_int, vp, ctypes.c_int, u64, ctypes.c_int, ctypes.c_int, vp]),
+    "sb_group_batch_apply_key": (ctypes.c_int, [vp, ctypes.c_int, vp, ctypes.c_int, u64, vp, vp, ctypes.c_int, vp]),
     "sb_groth16_load": (ctypes.c_int, [vp, vp, u64, ctypes.POINTER(u64)]),
     "sb_groth16_load_sharded": (ctypes.c_int, [vp, vp, u64, ctypes.c_int, ctypes.c_int, ctypes.POINTER(u64)]),
     "sb_groth16_load_file": (ctypes.c_int, [vp, ctypes.c_char_p, ctypes.POINTER(u64)]),

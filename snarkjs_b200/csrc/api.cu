@@ -22,6 +22,7 @@
 #include "msm.cuh"
 #include "msm_entry.h"
 #include "fr_entry.h"
+#include "gfft_entry.h"
 
 using namespace sb;
 namespace sb { double calibrate(int what, cudaStream_t stream); extern int g_ntt_tile_log; }
@@ -48,10 +49,12 @@ struct GroupOps {
     void (*times)(const uint8_t*, const uint8_t*, int, uint8_t*);
     int (*gen_points)(const uint8_t*, uint64_t, uint64_t, void*, cudaStream_t);
     int (*precompute)(const void*, uint64_t, int, int, void*, cudaStream_t);
+    int (*gfft)(const void*, int, uint64_t, int, const void*, const void*, int, void*, void*, cudaStream_t, int*);
+    int (*gapply)(const void*, int, const void*, uint64_t, int, void*, cudaStream_t);
     uint32_t xyzz_bytes;
     uint32_t aff_bytes;
 };
-#define SB_GROUP_OPS(NAME, AFF) GroupOps{NAME##_buckets, NAME##_combine, NAME##_add, NAME##_to_jacobian, NAME##_to_affine, NAME##_from_affine, NAME##_times, NAME##_gen_points, NAME##_precompute, NAME##_xyzz_bytes(), AFF}
+#define SB_GROUP_OPS(NAME, AFF) GroupOps{NAME##_buckets, NAME##_combine, NAME##_add, NAME##_to_jacobian, NAME##_to_affine, NAME##_from_affine, NAME##_times, NAME##_gen_points, NAME##_precompute, NAME##_gfft, NAME##_gapply, NAME##_xyzz_bytes(), AFF}
 
 struct NttTab { DevBuf lo, hi; int h = 0; };
 struct PreTab { DevBuf lo, hi; int h = 0; std::string key; };
@@ -279,6 +282,11 @@ const void* get_ninv(sb_ctx* c, int L) {
         it = c->ninv.find(L);
     }
     return it->second.p;
+}
+
+// plain (non-Montgomery) n^-1 for n = 2^L: the group iFFT scalar
+template <class P> void ninv_plain_bytes(int L, uint8_t* out) {
+    Fp<P> a; ninv_bytes<P>(L, (uint8_t*)&a); a = Fp<P>::from_mont(a); memcpy(out, &a, 32);
 }
 
 // apply-key tables for (n, first, inc): lo[e] = inc^e, hi[e] = first * inc^(e 2^h)
@@ -706,6 +714,92 @@ int sb_qap_join_abc(sb_ctx* c, const uint8_t* a, const uint8_t* b, const uint8_t
     int rc = fr_join_abc(c->curve, da, db, dc, dout, n, c->stream); c->launches++;
     if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_join_abc");
     CU(c, d2h(c, out, dout, n * 32));
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------- group FFT
+// plain Fr values first * inc^i, i < n, into d_out (d_tmp: n more elements): the apply-key kernel over Montgomery ones,
+// then out of Montgomery form (first, inc Montgomery)
+static int fr_powers_plain(sb_ctx* c, uint64_t n, const uint8_t* first, const uint8_t* inc, void* d_tmp, void* d_out) {
+    FrPre pre; int rc = get_pre(c, n, first, inc, &pre); if (rc) return rc;
+    uint8_t* o = (uint8_t*)d_out;
+    CU(c, cudaMemcpyAsync(o, c->roots[0].data(), 32, cudaMemcpyHostToDevice, c->stream));        // w[0] = Montgomery one
+    for (uint64_t k = 1; k < n; k *= 2) CU(c, cudaMemcpyAsync(o + k * 32, o, std::min(k, n - k) * 32, cudaMemcpyDeviceToDevice, c->stream));
+    rc = fr_apply_key(c->curve, d_out, d_tmp, n, &pre, c->stream); c->launches++;
+    if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_apply_key");
+    rc = fr_convert(c->curve, d_tmp, d_out, n, 0, c->stream); c->launches++;
+    if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_convert");
+    return 0;
+}
+static void* io_get(sb_ctx* c, int i, uint64_t bytes, int* rc) {
+    void* p = c->io[i].get(bytes);
+    if (!p) *rc = fail(c, SB_ERR_NOMEM, "out of device memory (" + std::to_string(bytes) + " bytes)");
+    return p;
+}
+static int group_ops(sb_ctx* c, int group, const GroupOps** G) {
+    if (!c || (group != SB_G1 && group != SB_G2)) return c ? fail(c, SB_ERR_ARG, "invalid group") : SB_ERR_ARG;
+    *G = group == SB_G1 ? &c->g1 : &c->g2;
+    return 0;
+}
+
+int sb_group_fft(sb_ctx* c, int group, const uint8_t* in, int in_jac, uint64_t n, int inverse, int out_jac, uint8_t* out) { SB_LOCK(c);
+    const GroupOps* G; int rc = group_ops(c, group, &G); if (rc) return rc;
+    if (n == 0 || (n & (n - 1))) return fail(c, SB_ERR_ARG, "fft must be multiple of 2");
+    int L = 0; while (((uint64_t)1 << L) < n) L++;
+    if (L > c->fr_s) return fail(c, SB_ERR_ARG, "fft size exceeds the 2-adicity of Fr (fftExt path not supported)");
+    cudaSetDevice(c->device);
+    const uint64_t n8 = G->aff_bytes / 2, sin = (in_jac ? 3 : 2) * n8, sout = (out_jac ? 3 : 2) * n8, ntw = std::max<uint64_t>(n / 2, 1);
+    uint8_t* d_io = (uint8_t*)io_get(c, 0, n * std::max(sin, sout), &rc);
+    void* d_pts = d_io ? io_get(c, 1, n * G->xyzz_bytes, &rc) : nullptr;
+    uint8_t* d_tw = d_pts ? (uint8_t*)io_get(c, 2, (ntw + 1) * 32, &rc) : nullptr;
+    void* d_tmp = d_tw ? io_get(c, 3, ntw * 32, &rc) : nullptr;
+    if (!d_tmp) return rc;
+    tick(c, 0);
+    CU(c, h2d(c, d_io, in, n * sin));
+    tick(c, 1);
+    if (L > 1) { rc = fr_powers_plain(c, n / 2, c->roots[0].data(), c->roots[L].data(), d_tmp, d_tw); if (rc) return rc; }
+    uint8_t* d_ninv = nullptr;
+    if (inverse) {
+        uint8_t b[32];
+        if (c->curve == SB_BN254) ninv_plain_bytes<BnFr>(L, b); else ninv_plain_bytes<BlsFr>(L, b);
+        d_ninv = d_tw + ntw * 32;
+        CU(c, cudaMemcpyAsync(d_ninv, b, 32, cudaMemcpyHostToDevice, c->stream));
+    }
+    int launches = 0;
+    rc = G->gfft(d_io, in_jac, n, L, d_tw, d_ninv, out_jac, d_pts, d_io, c->stream, &launches);
+    c->launches += launches;
+    if (rc) return cuda_fail(c, (cudaError_t)rc, "group fft");
+    tick(c, 2);
+    CU(c, d2h(c, out, d_io, n * sout));
+    tick(c, 3);
+    CU(c, cudaStreamSynchronize(c->stream));
+    c->last_ms[0] = elapsed(c, 0, 3); c->last_ms[1] = elapsed(c, 0, 1); c->last_ms[2] = elapsed(c, 1, 2); c->last_ms[3] = elapsed(c, 2, 3);
+    return 0;
+}
+
+int sb_group_batch_apply_key(sb_ctx* c, int group, const uint8_t* in, int in_jac, uint64_t n, const uint8_t first[32],
+                             const uint8_t inc[32], int out_jac, uint8_t* out) { SB_LOCK(c);
+    const GroupOps* G; int rc = group_ops(c, group, &G); if (rc) return rc;
+    c->last_ms[0] = 0;
+    if (n == 0) return 0;
+    cudaSetDevice(c->device);
+    const uint64_t n8 = G->aff_bytes / 2, sin = (in_jac ? 3 : 2) * n8, sout = (out_jac ? 3 : 2) * n8;
+    void* d_in = io_get(c, 0, n * sin, &rc);
+    void* d_out = d_in ? io_get(c, 1, n * sout, &rc) : nullptr;
+    void* d_sc = d_out ? io_get(c, 2, n * 32, &rc) : nullptr;
+    void* d_tmp = d_sc ? io_get(c, 3, n * 32, &rc) : nullptr;
+    if (!d_tmp) return rc;
+    tick(c, 0);
+    CU(c, h2d(c, d_in, in, n * sin));
+    tick(c, 1);
+    rc = fr_powers_plain(c, n, first, inc, d_tmp, d_sc); if (rc) return rc;
+    rc = G->gapply(d_in, in_jac, d_sc, n, out_jac, d_out, c->stream); c->launches++;
+    if (rc) return cuda_fail(c, (cudaError_t)rc, "group batchApplyKey");
+    tick(c, 2);
+    CU(c, d2h(c, out, d_out, n * sout));
+    tick(c, 3);
+    CU(c, cudaStreamSynchronize(c->stream));
+    c->last_ms[0] = elapsed(c, 0, 3); c->last_ms[1] = elapsed(c, 0, 1); c->last_ms[2] = elapsed(c, 1, 2); c->last_ms[3] = elapsed(c, 2, 3);
     return 0;
 }
 

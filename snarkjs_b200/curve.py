@@ -115,6 +115,7 @@ class Group:
         one = (1 << (8 * n8q)) % (_Q[(n8q, )])
         z = bytes(self.n8)
         self.zero = z + one.to_bytes(n8q, "little") + bytes(self.n8 - n8q) + z     # (0, 1, 0)
+        self._s = ctx.lib.sb_fr_root(ctx.h, 0, _ptr(np.empty(32, np.uint8)))     # Fr.s
 
     def multiExpAffine(self, buffBases, buffScalars, logger=None, logText=""):
         b, s = _arr(buffBases), _arr(buffScalars)
@@ -127,6 +128,52 @@ class Group:
         out = np.empty(self.sJacobian, np.uint8)
         fn = self._c.lib.sb_msm_g1_affine if self.gid == 1 else self._c.lib.sb_msm_g2_affine
         self._c.check(fn(self._c.h, _ptr(b), _ptr(s), ss, n, _ptr(out)))
+        return out
+
+    def _size(self, t: str) -> int:
+        return self.sJacobian if t == "jacobian" else self.sAffine
+
+    def _fft(self, buff, inverse, inType, outType):
+        a = _arr(buff)
+        sin, sout = self._size(inType or "affine"), self._size(outType or "affine")
+        n = a.size // sin
+        if n * sin != a.size or n == 0 or n & (n - 1):
+            raise SbError("fft must be multiple of 2")          # build/snarkjs.js:14745-14747
+        out = np.empty(n * sout, np.uint8)
+        self._c.check(self._c.lib.sb_group_fft(self._c.h, self.gid, _ptr(a), int(sin == self.sJacobian), n, int(inverse),
+                                               int(sout == self.sJacobian), _ptr(out)))
+        return out
+
+    def fft(self, buff, inType="affine", outType="affine", logger=None, loggerTxt=""):
+        """G.fft (build/snarkjs.js:15101-15103); Jacobian output is normalised to Z = 1 (infinity (0,1,0))."""
+        return self._fft(buff, False, inType, outType)
+
+    def ifft(self, buff, inType="affine", outType="affine", logger=None, loggerTxt=""):
+        """G.ifft (build/snarkjs.js:15105-15107)."""
+        return self._fft(buff, True, inType, outType)
+
+    def lagrangeEvaluations(self, buff, inType="affine", outType="affine", logger=None, loggerTxt=""):
+        """G.lagrangeEvaluations (build/snarkjs.js:15109-15176): the ifft for log2(n) <= Fr.s; log2(n) = Fr.s + 1 (the
+        reference's two-half path) is refused by the library like Fr.fft's fftExt path."""
+        sin = self._size(inType or "affine")
+        nbytes = buff.nbytes if isinstance(buff, np.ndarray) else _arr(buff).size
+        n = nbytes // sin
+        bits = max(n.bit_length() - 1, 0)
+        if (1 << bits) * sin != nbytes:
+            raise SbError("lagrangeEvaluations invalid Input size")
+        if bits > self._s + 1:
+            raise SbError("lagrangeEvaluations input too big")
+        return self.ifft(buff, inType, outType, logger, loggerTxt)
+
+    def batchApplyKey(self, buff, first: bytes, inc: bytes, inType="affine", outType="affine"):
+        """G.batchApplyKey (build/snarkjs.js:14268-14385): out[i] = in[i] * first * inc^i; first / inc Montgomery Fr;
+        the point count is floor(bytes / point size)."""
+        a = _arr(buff)
+        sin, sout = self._size(inType or "affine"), self._size(outType or "affine")
+        n = a.size // sin
+        out = np.empty(n * sout, np.uint8)
+        self._c.check(self._c.lib.sb_group_batch_apply_key(self._c.h, self.gid, _ptr(a), int(sin == self.sJacobian), n,
+                                                           bytes(first), bytes(inc), int(sout == self.sJacobian), _ptr(out)))
         return out
 
     def toAffine(self, jac) -> np.ndarray:
