@@ -207,7 +207,8 @@ float sb_last_ms(sb_ctx* ctx, int which);
 /* counters of the last MSM / prove call: 0/1 = summed device time (ms) of the G1 / G2 bucket-accumulation kernel
  * launches, 2/3 = number of those launches, 4/5 = (scalar digit, point) entries they consumed; 8..15 = device time (ms) per
  * kernel class: digits + radix sort, G1 accumulation, G2 accumulation, head folding, bucket reduction + window sums,
- * QAP rows, NTT passes, joinABC (meaningful per class when the call ran serialised, sb_set_tuning(2, 1)). */
+ * QAP rows, NTT passes, joinABC (meaningful per class when the call ran serialised, sb_set_tuning(2, 1)); 16/17 = the part
+ * of 11/12 (head folding / bucket reduction) spent in G2 MSMs. */
 double sb_last_stat(sb_ctx* ctx, int which);
 /* integer-pipe calibration on this device: what = 0 -> IMAD.WIDE.U32 per second, 1 -> register-resident BN254 Fq
  * Montgomery multiplies per second (the modmul-bound roofline denominators, SURVEY.md §8d). */

@@ -118,7 +118,7 @@ struct sb_ctx {
     std::vector<uint8_t> nqr, shift;
     std::vector<uint8_t> gen1, gen2;            // affine generators, Montgomery
     cudaEvent_t prof_ev[256];
-    double stat[16] = {0};                       // see sb_last_stat
+    double stat[18] = {0};                       // see sb_last_stat
     // multi-GPU (sb_comm_init_rank): one NCCL rank per context
     ncclComm_t comm = nullptr; int rank = 0, world = 1;
     void* d_xchg = nullptr; uint8_t* h_xchg = nullptr;   // partial exchange: world x partial bytes (device / pinned)
@@ -355,6 +355,8 @@ void prof_end(sb_ctx* c) {
         else if (g == PROF_ACC_G2) { c->stat[1] += ms; c->stat[3] += 1; c->stat[10] += ms; }
         else if (g == PROF_SORT) c->stat[8] += ms;
         else if (g >= PROF_FOLD && g <= PROF_JOIN) c->stat[11 + (g - PROF_FOLD)] += ms;
+        else if (g == PROF_FOLD_G2) { c->stat[11] += ms; c->stat[16] += ms; }
+        else if (g == PROF_REDUCE_G2) { c->stat[12] += ms; c->stat[17] += ms; }
     }
     c->stats.ev = nullptr; c->stats.used = 0;
 }
@@ -824,7 +826,7 @@ int sb_set_tuning(int key, int value) {
     default: return SB_ERR_ARG;
     }
 }
-double sb_last_stat(sb_ctx* c, int which) { SB_LOCK(c); return (c && which >= 0 && which < 16) ? c->stat[which] : 0.0; }
+double sb_last_stat(sb_ctx* c, int which) { SB_LOCK(c); return (c && which >= 0 && which < 18) ? c->stat[which] : 0.0; }
 double sb_calibrate(sb_ctx* c, int what) { SB_LOCK(c); if (!c) return -1; cudaSetDevice(c->device); return calibrate(what, c->stream); }
 int sb_gen_points(sb_ctx* c, int group, uint64_t seed, uint64_t n, uint8_t* out) { SB_LOCK(c);
     if (!c || (group != SB_G1 && group != SB_G2)) return SB_ERR_ARG;

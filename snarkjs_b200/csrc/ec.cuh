@@ -121,7 +121,28 @@ template <class F> struct XYZZ {
         else Y3 = F::sub(F::mul_i(R, F::sub(Q, X3)), F::mul_i(y, PPP));
         x = X3; y = Y3; zz = F::mul_i(zz, PP); zzz = F::mul_i(zzz, PPP);
     }
-    // acc += q   (add-2008-s)
+    // acc += q   (add-2008-s), for the device reduction kernels: the same formulas and special cases as add() below, hence
+    // the same bytes, with the force-inlined multiplies.  q's zz and zzz enter their last products first, so they die
+    // before the bulk of the addition.
+    SB_HD void add_i(const XYZZ& q) {
+        if (q.is_inf()) return;
+        if (is_inf()) { *this = q; return; }
+        F U1 = F::mul_i(x, q.zz), S1 = F::mul_i(y, q.zzz);
+        F ZZ = F::mul_i(zz, q.zz), ZZZ = F::mul_i(zzz, q.zzz);
+        F Pp = F::sub(F::mul_i(q.x, zz), U1), R = F::sub(F::mul_i(q.y, zzz), S1);
+        if (Pp.is_zero()) {
+            if (R.is_zero()) *this = dbl(*this);
+            else *this = inf();
+            return;
+        }
+        F PP = F::sqr_i(Pp), PPP = F::mul_i(Pp, PP), Q = F::mul_i(U1, PP);
+        F X3 = F::sub(F::sub(F::sqr_i(R), PPP), F::dbl(Q));
+        F Y3;
+        if constexpr (F::HAS_MUL2) Y3 = F::mul2_i(R, F::sub(Q, X3), F::neg(S1), PPP);   // R(Q - X3) - S1*PPP, one reduction
+        else Y3 = F::sub(F::mul_i(R, F::sub(Q, X3)), F::mul_i(S1, PPP));
+        x = X3; y = Y3; zz = F::mul_i(ZZ, PP); zzz = F::mul_i(ZZZ, PPP);
+    }
+    // acc += q   (add-2008-s): host code and the group FFT
     SB_HD void add(const XYZZ& q) {
         if (q.is_inf()) return;
         if (is_inf()) { *this = q; return; }

@@ -150,8 +150,8 @@ k_accumulate(const Affine<F>* __restrict__ bases, const uint32_t* __restrict__ k
 // INVALID in keys_out; longer runs (skewed scalars: giant buckets) keep their key and go to the k_fold cascade.
 // ------------------------------------------------------------------------------------------------
 static constexpr int MSM_SHORT_RUN = 8;
-template <class F>
-__global__ void __launch_bounds__(MSM_ACC_THREADS)
+template <class F, int MINB>
+__global__ void __launch_bounds__(MSM_ACC_THREADS, MINB)
 k_fold_short(const XYZZ<F>* __restrict__ heads, const uint32_t* __restrict__ keys_in, uint32_t* __restrict__ keys_out,
              const uint64_t* __restrict__ counts, XYZZ<F>* __restrict__ buckets) {
     const uint64_t M = counts[1];
@@ -171,7 +171,7 @@ k_fold_short(const XYZZ<F>* __restrict__ heads, const uint32_t* __restrict__ key
     keys_out[t] = is_short ? MSM_INVALID_KEY : k;
     if (!is_short || start != t) return;
     XYZZ<F> acc = load_vec(buckets + k);
-    for (uint64_t e = 0; e < len; e++) { XYZZ<F> p = load_vec(heads + t + e); acc.add(p); }
+    for (uint64_t e = 0; e < len; e++) { XYZZ<F> p = load_vec(heads + t + e); acc.add_i(p); }
     store_vec(buckets + k, acc);
 }
 
@@ -192,14 +192,14 @@ k_fold(const XYZZ<F>* __restrict__ in, const uint32_t* __restrict__ in_keys, con
     XYZZ<F> acc = XYZZ<F>::inf();
     uint32_t cur = in_keys[lo];
     bool first = !last;
-    auto flush = [&]() {
+    auto flush = [&]() __attribute__((always_inline)) {
         if (first) { store_vec(heads + t, acc); head_keys[t] = cur; first = false; }
-        else if (cur != MSM_INVALID_KEY) { XYZZ<F> b = load_vec(buckets + cur); b.add(acc); store_vec(buckets + cur, b); }
+        else if (cur != MSM_INVALID_KEY) { XYZZ<F> b = load_vec(buckets + cur); b.add_i(acc); store_vec(buckets + cur, b); }
     };
     for (uint64_t e = lo; e < hi; e++) {
         uint32_t k = in_keys[e];
         if (k != cur) { flush(); acc = XYZZ<F>::inf(); cur = k; }
-        if (k != MSM_INVALID_KEY) { XYZZ<F> p = load_vec(in + e); acc.add(p); }
+        if (k != MSM_INVALID_KEY) { XYZZ<F> p = load_vec(in + e); acc.add_i(p); }
     }
     flush();
 }
@@ -225,8 +225,8 @@ k_reduce(const XYZZ<F>* __restrict__ buckets, MsmGeom g, XYZZ<F>* __restrict__ p
         XYZZ<F> run = XYZZ<F>::inf(), sum = XYZZ<F>::inf();
         for (int b = (int)L - 1; b >= 0; b--) {
             XYZZ<F> p = load_vec(bk + b);
-            run.add(p);
-            sum.add(run);
+            run.add_i(p);
+            sum.add_i(run);
         }
         // part = sum + (j*L) * run   (double-and-add, MSB first)
         uint32_t k = j * L;
@@ -235,17 +235,17 @@ k_reduce(const XYZZ<F>* __restrict__ buckets, MsmGeom g, XYZZ<F>* __restrict__ p
             part = run;
             for (int bit = top - 1; bit >= 0; bit--) {
                 part = XYZZ<F>::dbl(part);
-                if ((k >> bit) & 1) part.add(run);
+                if ((k >> bit) & 1) part.add_i(run);
             }
         }
-        part.add(sum);
+        part.add_i(sum);
     }
     store_vec(sm + threadIdx.x, part);
     __syncthreads();
     for (uint32_t s = blockDim.x >> 1; s > 0; s >>= 1) {
         if (threadIdx.x < s) {
             XYZZ<F> a = load_vec(sm + threadIdx.x), b = load_vec(sm + threadIdx.x + s);
-            a.add(b);
+            a.add_i(b);
             store_vec(sm + threadIdx.x, a);
         }
         __syncthreads();
@@ -260,11 +260,11 @@ k_window_sum(const XYZZ<F>* __restrict__ partials, uint32_t per_window, XYZZ<F>*
     extern __shared__ uint4 smem_raw[];
     XYZZ<F>* sm = reinterpret_cast<XYZZ<F>*>(smem_raw);
     XYZZ<F> acc = XYZZ<F>::inf();
-    for (uint32_t i = threadIdx.x; i < per_window; i += 32) { XYZZ<F> p = load_vec(partials + (uint64_t)blockIdx.x * per_window + i); acc.add(p); }
+    for (uint32_t i = threadIdx.x; i < per_window; i += 32) { XYZZ<F> p = load_vec(partials + (uint64_t)blockIdx.x * per_window + i); acc.add_i(p); }
     store_vec(sm + threadIdx.x, acc);
     __syncwarp();
     for (uint32_t s = 16; s > 0; s >>= 1) {
-        if (threadIdx.x < s) { XYZZ<F> a = load_vec(sm + threadIdx.x), b = load_vec(sm + threadIdx.x + s); a.add(b); store_vec(sm + threadIdx.x, a); }
+        if (threadIdx.x < s) { XYZZ<F> a = load_vec(sm + threadIdx.x), b = load_vec(sm + threadIdx.x + s); a.add_i(b); store_vec(sm + threadIdx.x, a); }
         __syncwarp();
     }
     if (threadIdx.x == 0) store_vec(out + blockIdx.x, load_vec(sm));
@@ -286,12 +286,11 @@ k_window_sum(const XYZZ<F>* __restrict__ partials, uint32_t per_window, XYZZ<F>*
 //   k_ws_final   one CTA per window: the same warp routine over the chunk totals, then the power-of-two weights
 //                (2^m, 2^5) by doublings of single points.
 // ------------------------------------------------------------------------------------------------
-template <class F> __device__ __noinline__ void padd(XYZZ<F>& a, const XYZZ<F>& b) { a.add(b); }
 
 struct AxisJob { const void* in; void* out; uint64_t total; uint32_t S; uint32_t log_inner; };
 
-template <class F>
-__global__ void __launch_bounds__(128)
+template <class F, int MINB>
+__global__ void __launch_bounds__(128, MINB)
 k_axis_sum(AxisJob j0, AxisJob j1) {
     const AxisJob j = blockIdx.y ? j1 : j0;
     const uint64_t gid = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
@@ -300,7 +299,7 @@ k_axis_sum(AxisJob j0, AxisJob j1) {
     const XYZZ<F>* p = (const XYZZ<F>*)j.in + ((o * j.S) << j.log_inner) + i;
     XYZZ<F> acc = load_vec(p);
 #pragma unroll 1
-    for (uint32_t s = 1; s < j.S; s++) { XYZZ<F> v = load_vec(p + ((uint64_t)s << j.log_inner)); acc.add(v); }
+    for (uint32_t s = 1; s < j.S; s++) { XYZZ<F> v = load_vec(p + ((uint64_t)s << j.log_inner)); acc.add_i(v); }
     store_vec((XYZZ<F>*)j.out + gid, acc);
 }
 
@@ -316,17 +315,17 @@ template <class F> __device__ __forceinline__ XYZZ<F> shfl_down_pt(const XYZZ<F>
 template <class F> __device__ __forceinline__ void warp_weighted_sum(XYZZ<F> v, XYZZ<F>& T, XYZZ<F>& W) {
     const int lane = threadIdx.x & 31;
 #pragma unroll 1
-    for (int d = 1; d < 32; d <<= 1) { XYZZ<F> o = shfl_down_pt<F>(v, d); if (lane + d < 32) v.add(o); }   // suffix sums
+    for (int d = 1; d < 32; d <<= 1) { XYZZ<F> o = shfl_down_pt<F>(v, d); if (lane + d < 32) v.add_i(o); }   // suffix sums
     T = v;
     XYZZ<F> x = lane ? v : XYZZ<F>::inf();
 #pragma unroll 1
-    for (int d = 16; d >= 1; d >>= 1) { XYZZ<F> o = shfl_down_pt<F>(x, d); if (lane < d) x.add(o); }
+    for (int d = 16; d >= 1; d >>= 1) { XYZZ<F> o = shfl_down_pt<F>(x, d); if (lane < d) x.add_i(o); }
     W = x;
 }
 template <class F> __device__ __forceinline__ XYZZ<F> warp_sum(XYZZ<F> x) {
     const int lane = threadIdx.x & 31;
 #pragma unroll 1
-    for (int d = 16; d >= 1; d >>= 1) { XYZZ<F> o = shfl_down_pt<F>(x, d); if (lane < d) x.add(o); }
+    for (int d = 16; d >= 1; d >>= 1) { XYZZ<F> o = shfl_down_pt<F>(x, d); if (lane < d) x.add_i(o); }
     return x;
 }
 
@@ -386,7 +385,7 @@ k_axis_tree(AxisJob j0, AxisJob j1) {
     const XYZZ<F>* p = (const XYZZ<F>*)j.in + ((o * j.S) << j.log_inner) + i;
     XYZZ<F> acc = XYZZ<F>::inf();
 #pragma unroll 1
-    for (uint32_t s = lane; s < j.S; s += 32) { XYZZ<F> v = load_vec(p + ((uint64_t)s << j.log_inner)); acc.add(v); }
+    for (uint32_t s = lane; s < j.S; s += 32) { XYZZ<F> v = load_vec(p + ((uint64_t)s << j.log_inner)); acc.add_i(v); }
     acc = warp_sum<F>(acc);
     if (lane == 0) store_vec((XYZZ<F>*)j.out + wid, acc);
 }
@@ -506,7 +505,8 @@ struct MsmLaunchStats {
     // optional profiling: event pairs recorded around kernel groups (tag = PROF_* below; accumulation uses cur_tag)
     cudaEvent_t* ev = nullptr; int nev = 0; int used = 0; int tag[128] = {0}; int cur_tag = 0;
 };
-enum { PROF_ACC_G1 = 1, PROF_ACC_G2 = 2, PROF_SORT = 3, PROF_FOLD = 4, PROF_REDUCE = 5, PROF_QAP = 6, PROF_NTT = 7, PROF_JOIN = 8 };
+enum { PROF_ACC_G1 = 1, PROF_ACC_G2 = 2, PROF_SORT = 3, PROF_FOLD = 4, PROF_REDUCE = 5, PROF_QAP = 6, PROF_NTT = 7, PROF_JOIN = 8,
+       PROF_FOLD_G2 = 9, PROF_REDUCE_G2 = 10 };
 // one event pair around a group of launches on `st`; a no-op unless profiling is armed (api.cu prof_begin)
 struct ProfScope {
     MsmLaunchStats* s; cudaStream_t st; int idx = -1;
@@ -568,6 +568,13 @@ int msm_buckets(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& scratc
     XYZZ<F>* partials = (XYZZ<F>*)(base + o_part);
     uint32_t* hkM = (uint32_t*)(base + o_hkM);
     int launches = 0;
+    const bool g2 = stats && stats->cur_tag == PROF_ACC_G2;     // the tail's profiling tags name the MSM's group
+    // minBlocksPerSM of the two wide tail kernels (k_fold_short, k_axis_sum), per coordinate field as for k_accumulate
+    // below.  ptxas, sm_90a, registers of k_fold_short / k_axis_sum: BN254 G1 124 / 124, BLS12-381 G1 190 / 190, BN254 G2
+    // 248 / 242, all without spills; BLS12-381 G2 255 / 255 with 132 / 52 B of spill stores, which no launch bound can
+    // remove (255 is the per-thread cap).  H100 at 400 W: a 2^20 BLS12-381 G2 MSM 26.5 ms, 26.6 with the
+    // out-of-line additions of XYZZ::add.
+    constexpr int TAIL_MINB = sizeof(F) > 32 ? 2 : 4;
     cudaMemsetAsync(buckets, 0, nbuckets * sizeof(XYZZ<F>), stream);
     if (heads0) {
         ProfScope prof(stats, stats ? stats->cur_tag : 0, stream);
@@ -587,8 +594,8 @@ int msm_buckets(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& scratc
         if (tail_stream && tail_stream != stream && ev_acc) {
             cudaEventRecord(ev_acc, stream); cudaStreamWaitEvent(tail_stream, ev_acc, 0); stream = tail_stream;
         }
-        ProfScope pfold(stats, PROF_FOLD, stream);
-        k_fold_short<F><<<(unsigned)((heads0 + MSM_ACC_THREADS - 1) / MSM_ACC_THREADS), MSM_ACC_THREADS, 0, stream>>>(
+        ProfScope pfold(stats, g2 ? PROF_FOLD_G2 : PROF_FOLD, stream);
+        k_fold_short<F, TAIL_MINB><<<(unsigned)((heads0 + MSM_ACC_THREADS - 1) / MSM_ACC_THREADS), MSM_ACC_THREADS, 0, stream>>>(
             headsA, hkA, hkM, s.counts, buckets); launches++;
         // fold cascade: level l consumes counts[l] heads (upper bound m on the host, exact count on the device)
         uint64_t m = heads0; int level = 1;
@@ -605,7 +612,7 @@ int msm_buckets(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& scratc
         pfold.end();
     }
     if (!heads0 && tail_stream && tail_stream != stream && ev_acc) { cudaEventRecord(ev_acc, stream); cudaStreamWaitEvent(tail_stream, ev_acc, 0); stream = tail_stream; }
-    ProfScope pred(stats, PROF_REDUCE, stream);
+    ProfScope pred(stats, g2 ? PROF_REDUCE_G2 : PROF_REDUCE, stream);
     const WsPlan wp = ws_plan(g);
     if (wp.ok && !g_msm_force_reduce) {
         // axis sums (rows and columns of one level per launch), then the warp-shuffle weighted sums
@@ -619,7 +626,7 @@ int msm_buckets(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& scratc
             if (wp.br[l]) { rr -= wp.br[l]; jr = AxisJob{rin, rowb[l & 1], (uint64_t)nbuckets >> (wp.er - rr), 1u << wp.br[l], (uint32_t)rr}; rin = rowb[l & 1]; }
             if (wp.bc[l]) { rc -= wp.bc[l]; jc = AxisJob{cin, colb[l & 1], (uint64_t)nbuckets >> (wp.ec - rc), 1u << wp.bc[l], (uint32_t)wp.m}; cin = colb[l & 1]; }
             const uint64_t mx = jr.total > jc.total ? jr.total : jc.total;
-            if (l == 0) k_axis_sum<F><<<dim3((unsigned)((mx + 127) / 128), 2), 128, 0, stream>>>(jr, jc);
+            if (l == 0) k_axis_sum<F, TAIL_MINB><<<dim3((unsigned)((mx + 127) / 128), 2), 128, 0, stream>>>(jr, jc);
             else k_axis_tree<F><<<dim3((unsigned)((mx + 3) / 4), 2), 128, 0, stream>>>(jr, jc);
             launches++;
         }
