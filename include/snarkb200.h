@@ -231,6 +231,22 @@ int sb_set_tuning(int key, int value);
  * on the GPU; the same points as the CPU oracle's incremental generator (oracle/snark_oracle.cpp or_gen_points), see msm.cuh. */
 int sb_gen_points(sb_ctx* ctx, int group, uint64_t seed, uint64_t n, uint8_t* out);
 int sb_generator(sb_ctx* ctx, int group, uint8_t* out_affine);
+/* test hook: one field primitive of the device arithmetic (csrc/fp.cuh, csrc/ec.cuh) over n records, as compiled for the
+ * GPU.  The field does not depend on the context's curve; the context supplies the device, stream and buffers.
+ *   field: 0 BN254 Fq, 1 BN254 Fr, 2 BLS12-381 Fq, 3 BLS12-381 Fr, 4 BN254 Fq2, 5 BLS12-381 Fq2
+ *   in: n records of k little-endian elements (N limbs of 32 bits each: 32 or 48 bytes; an Fq2 element is c0 || c1),
+ *   out: n results.  Values are raw residues: "Montgomery" operations compute with R = 2^(32N).
+ *   op  fields  in -> out
+ *    0  0-3     a, b -> a + b                      7  0-3   T (2N limbs, T < p*R) -> T*R^-1
+ *    1  0-3     a, b -> a - b                      8  0-3   a -> a*R (to_mont; any a < 2^(32N))
+ *    2  0-3     a -> -a                            9  0-3   a -> a*R^-1 (from_mont; any a < 2^(32N))
+ *    3  0-3     a -> 2a                           10  0-3   a -> R^2*a^-1, 0 -> 0 (binary inversion)
+ *    4  0-3     a, b -> a*b*R^-1 (mul)            11  0-3   a -> R^2*a^-1, 0 -> 0 (a^(p-2))
+ *    5  0-2     x, y, u, v -> (x*y + u*v)*R^-1    12  4-5   x, y -> x*y*R^-1 (dual-product schoolbook)
+ *               (mul2: not on BLS12-381 Fr)       13  4-5   x, y -> x*y*R^-1 (lazy Karatsuba)
+ *    6  0-3     a, b -> a*b (2N limbs)            14  4-5   x -> x^2*R^-1      15  4-5   x -> R^2*x^-1, 0 -> 0
+ * Operands other than to_mont / from_mont inputs must be below p.  Any other (field, op) pair is SB_ERR_ARG. */
+int sb_field_eval(sb_ctx* ctx, int field, int op, const uint8_t* in, uint64_t n, uint8_t* out);
 int sb_sync(sb_ctx* ctx);
 
 #ifdef __cplusplus

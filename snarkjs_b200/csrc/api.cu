@@ -23,6 +23,7 @@
 #include "msm_entry.h"
 #include "fr_entry.h"
 #include "gfft_entry.h"
+#include "field_entry.h"
 
 using namespace sb;
 namespace sb { double calibrate(int what, cudaStream_t stream); extern int g_ntt_tile_log; }
@@ -837,6 +838,20 @@ int sb_gen_points(sb_ctx* c, int group, uint64_t seed, uint64_t n, uint8_t* out)
     int rc = G.gen_points(group == SB_G1 ? c->gen1.data() : c->gen2.data(), seed, n, d, c->stream); c->launches++;
     if (rc) return cuda_fail(c, (cudaError_t)rc, "gen_points");
     CU(c, d2h(c, out, d, n * G.aff_bytes));
+    return 0;
+}
+int sb_field_eval(sb_ctx* c, int field, int op, const uint8_t* in, uint64_t n, uint8_t* out) { SB_LOCK(c);
+    if (!c) return SB_ERR_ARG;
+    int wi, wo;
+    if (field_eval_shape(field, op, &wi, &wo)) return fail(c, SB_ERR_ARG, "sb_field_eval: op " + std::to_string(op) + " is not defined on field " + std::to_string(field));
+    if (n == 0) return 0;
+    cudaSetDevice(c->device);
+    void* d_in = c->io[0].get(n * wi * 4); void* d_out = c->io[1].get(n * wo * 4);
+    if (!d_in || !d_out) return fail(c, SB_ERR_NOMEM, "out of device memory");
+    CU(c, h2d(c, d_in, in, n * wi * 4));
+    int rc = field_eval(field, op, d_in, d_out, n, c->stream); c->launches++;
+    if (rc) return cuda_fail(c, (cudaError_t)rc, "field_eval");
+    CU(c, d2h(c, out, d_out, n * wo * 4));
     return 0;
 }
 int sb_generator(sb_ctx* c, int group, uint8_t* out) { SB_LOCK(c);

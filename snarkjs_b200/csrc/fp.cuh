@@ -416,7 +416,10 @@ _Pragma("unroll")
     }
     SB_HD static Fp mul_i(const Fp& a, const Fp& b) { return mul(a, b); }
     SB_HD static Fp sqr_i(const Fp& a) { return mul(a, a); }
-    SB_HD static Fp to_mont(const Fp& a) { return mul(a, r2()); }
+    // a*R mod p for any a < R, not only a < p: the conversion kernels take the caller's bytes unchecked.  The CIOS rows
+    // multiply the first operand by one word of the second, and their running value stays below first + p; with
+    // R^2 mod p first that is < 2p < R, while a first operand near R would carry out of the top limb.
+    SB_HD static Fp to_mont(const Fp& a) { return mul(r2(), a); }
 
 #ifndef __CUDA_ARCH__
     // Host-side multiply (final proof assembly, window Horner): plain word-serial Montgomery with 64-bit
