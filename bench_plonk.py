@@ -52,7 +52,7 @@ def host_flow_lib(proto: str):
     os.makedirs(out_dir, exist_ok=True)
     so = os.path.join(out_dir, f"libhost{proto}_omp.so")
     deps = [src, os.path.join(ROOT, "tests", "host", "host_backend.h")] + [os.path.join(ROOT, "snarkjs_b200", "csrc", f) for f in
-                                                                             ("plonk_flow.h", "plonk.cuh", "fflonk_flow.h", "fflonk.cuh", "fp.cuh")]
+                                                                             ("plonk_flow.h", "plonk.cuh", "fflonk_flow.h", "fflonk.cuh", "fp.cuh", "zkey.h")]
     if not os.path.exists(so) or any(os.path.getmtime(d) > os.path.getmtime(so) for d in deps):
         subprocess.check_call(["g++", "-O3", "-march=native", "-fopenmp", "-std=c++17", "-shared", "-fPIC", "-o", so, src, "-ldl"])
     lib = ctypes.CDLL(so)

@@ -132,7 +132,7 @@ Napi::Value Groth16Prove(const Napi::CallbackInfo& info) {
   return Queue(info.Env(), c, 8 * n8q, [=](std::vector<uint8_t>& out) { return sb_groth16_prove(c, h, pw, nw, pr, ps, out.data()); }, {w, r, s});
 }
 
-// groth16LoadFile(ctx, path) -> handle: the zkey is streamed from disk through pinned buffers (sb_groth16_load_file), never
+// groth16LoadFile(ctx, path) -> handle: the zkey is mapped from disk and streamed to HBM (sb_groth16_load_file), never
 // materialised in the JS heap; groth16ProveWtns(ctx, handle, wtnsFileBytes, r, s, n8q) -> Promise<Buffer(8*n8q)>
 Napi::Value Groth16LoadFile(const Napi::CallbackInfo& info) {
   sb_ctx* c = ctx_of(info[0]); std::string path = info[1].As<Napi::String>().Utf8Value(); uint64_t h = 0;

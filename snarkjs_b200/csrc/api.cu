@@ -1,7 +1,6 @@
 // api.cu — the C ABI of libsnarkb200.so (include/snarkb200.h): context, device buffers, table caches, the
 // drop-in bulk operations, and the fused Groth16 prover.  Host-side orchestration only; kernels live in
 // msm*.cu / fr_kernels.cu.  There is no CPU fallback: without a CUDA device sb_create fails.
-#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <string>
@@ -24,6 +23,7 @@
 #include "fr_entry.h"
 #include "gfft_entry.h"
 #include "field_entry.h"
+#include "zkey.h"
 
 using namespace sb;
 namespace sb { double calibrate(int what, cudaStream_t stream); extern int g_ntt_tile_log; }
@@ -454,35 +454,6 @@ int msm_host_inputs(sb_ctx* c, int group, const uint8_t* bases, const void* d_ba
     return 0;
 }
 
-// ------------------------------------------------------------------------------------------------------------
-// binfile / zkey parsing (@iden3/binfileutils readBinFile 17468-17498; src/zkey_utils.js:229-259)
-// ------------------------------------------------------------------------------------------------------------
-struct Section { uint64_t pos = 0, len = 0; bool present = false; };
-int parse_binfile(sb_ctx* c, const uint8_t* d, uint64_t len, const char* magic, uint32_t max_version, std::map<uint32_t, Section>& secs) {
-    if (len < 12 || memcmp(d, magic, 4) != 0) return fail(c, SB_ERR_FORMAT, std::string(magic) + ": Invalid File format");
-    uint32_t ver, nsec; memcpy(&ver, d + 4, 4); memcpy(&nsec, d + 8, 4);
-    if (ver > max_version) return fail(c, SB_ERR_FORMAT, "Version not supported");
-    uint64_t pos = 12;
-    for (uint32_t i = 0; i < nsec; i++) {
-        if (len - pos < 12) return fail(c, SB_ERR_FORMAT, "Invalid file size");
-        uint32_t id; uint64_t sl; memcpy(&id, d + pos, 4); memcpy(&sl, d + pos + 4, 8); pos += 12;
-        if (sl > len - pos) return fail(c, SB_ERR_FORMAT, "Invalid file size");   // (not pos + sl > len: sl comes from the file and may wrap)
-        if (secs[id].present) return fail(c, SB_ERR_FORMAT, "Section Duplicated " + std::to_string(id));
-        secs[id].pos = pos; secs[id].len = sl; secs[id].present = true;
-        pos += sl;
-    }
-    if (pos != len) return fail(c, SB_ERR_FORMAT, "Invalid file size");
-    return 0;
-}
-
-bool modulus_matches(const uint8_t* p, uint32_t n8, int curve, bool scalar_field) {
-    uint32_t limbs[12] = {0};
-    if (curve == SB_BN254) { if (n8 != 32) return false; for (int i = 0; i < 8; i++) limbs[i] = scalar_field ? BnFr::p(i) : BnFq::p(i); }
-    else if (scalar_field) { if (n8 != 32) return false; for (int i = 0; i < 8; i++) limbs[i] = BlsFr::p(i); }
-    else { if (n8 != 48) return false; for (int i = 0; i < 12; i++) limbs[i] = BlsFq::p(i); }
-    return memcmp(p, limbs, n8) == 0;
-}
-
 void free_key(Groth16Key* k) {
     for (void* p : {k->tA, k->tB1, k->tB2, k->tC, k->tH, k->dA, k->dB1, k->dB2, k->dC, k->dH, (void*)k->d_rowptr, (void*)k->d_sig, k->d_coef, k->dW, k->dA_T, k->dB_T, k->dC_T, k->dTmp, k->dTmp2, k->dTmp3, k->dWsum})
         if (p) cudaFree(p);
@@ -866,155 +837,43 @@ int sb_dev_upload(sb_ctx* c, void* dst, const uint8_t* src, uint64_t bytes) { SB
 int sb_dev_download(sb_ctx* c, uint8_t* dst, const void* src, uint64_t bytes) { SB_LOCK(c); if (!c) return SB_ERR_ARG; cudaSetDevice(c->device); CU(c, d2h(c, dst, src, bytes)); return 0; }
 
 // ---------------------------------------------------------------------------------------------------- Groth16
-// A zkey comes either as a memory image (z != nullptr) or as a file streamed section by section: the small sections
-// (1, 2, 4) are read to the host, the base sections (5-9) go straight to HBM through two pinned staging buffers with
-// cudaMemcpyAsync overlapping the next fread (SURVEY §8f rank 2).
-struct ZkeySource {
-    const uint8_t* z = nullptr; uint64_t zlen = 0; FILE* f = nullptr;
-    std::vector<uint8_t> small[5];   // host copies of sections 1, 2, 4 when streaming
-};
-static int zkey_section_table(sb_ctx* c, ZkeySource& src, std::map<uint32_t, Section>& secs) {
-    if (src.z) return parse_binfile(c, src.z, src.zlen, "zkey", 2, secs);
-    uint8_t hd[12];
-    if (fseek(src.f, 0, SEEK_END)) return fail(c, SB_ERR_FORMAT, "zkey: seek failed");
-    const uint64_t flen = (uint64_t)ftell(src.f);
-    fseek(src.f, 0, SEEK_SET);
-    if (fread(hd, 1, 12, src.f) != 12 || memcmp(hd, "zkey", 4) != 0) return fail(c, SB_ERR_FORMAT, "zkey: Invalid File format");
-    uint32_t ver, nsec; memcpy(&ver, hd + 4, 4); memcpy(&nsec, hd + 8, 4);
-    if (ver > 2) return fail(c, SB_ERR_FORMAT, "Version not supported");
-    uint64_t pos = 12;
-    for (uint32_t i = 0; i < nsec; i++) {
-        if (fseek(src.f, (long)pos, SEEK_SET) || fread(hd, 1, 12, src.f) != 12) return fail(c, SB_ERR_FORMAT, "Invalid file size");
-        uint32_t id; uint64_t sl; memcpy(&id, hd, 4); memcpy(&sl, hd + 4, 8); pos += 12;
-        if (pos > flen || sl > flen - pos) return fail(c, SB_ERR_FORMAT, "Invalid file size");
-        if (secs[id].present) return fail(c, SB_ERR_FORMAT, "Section Duplicated " + std::to_string(id));
-        secs[id].pos = pos; secs[id].len = sl; secs[id].present = true; pos += sl;
-    }
-    if (pos != flen) return fail(c, SB_ERR_FORMAT, "Invalid file size");
-    return 0;
-}
-// host pointer to a small section
-static const uint8_t* zkey_host_section(ZkeySource& src, const std::map<uint32_t, Section>& secs, uint32_t id, int slot) {
-    const Section& s = secs.at(id);
-    if (src.z) return src.z + s.pos;
-    src.small[slot].resize(s.len ? s.len : 1);
-    if (fseek(src.f, (long)s.pos, SEEK_SET) || fread(src.small[slot].data(), 1, s.len, src.f) != s.len) return nullptr;
-    return src.small[slot].data();
-}
-// section bytes [off, off+len) -> device
-static cudaError_t zkey_to_device(sb_ctx* c, ZkeySource& src, const std::map<uint32_t, Section>& secs, uint32_t id, uint64_t off, uint64_t len, void* dst) {
-    if (!len) return cudaSuccess;
-    const Section& s = secs.at(id);
-    if (src.z) return cudaMemcpy(dst, src.z + s.pos + off, len, cudaMemcpyHostToDevice);
-    const size_t CH = 16u << 20;
-    uint8_t* pin[2] = {nullptr, nullptr}; cudaEvent_t ev[2];
-    cudaError_t e = cudaHostAlloc((void**)&pin[0], CH, cudaHostAllocDefault); if (e != cudaSuccess) return e;
-    e = cudaHostAlloc((void**)&pin[1], CH, cudaHostAllocDefault); if (e != cudaSuccess) { cudaFreeHost(pin[0]); return e; }
-    cudaEventCreateWithFlags(&ev[0], cudaEventDisableTiming); cudaEventCreateWithFlags(&ev[1], cudaEventDisableTiming);
-    if (fseek(src.f, (long)(s.pos + off), SEEK_SET)) e = cudaErrorUnknown;
-    uint64_t done = 0; int b = 0; bool used[2] = {false, false};
-    while (e == cudaSuccess && done < len) {
-        const size_t n = (size_t)std::min<uint64_t>(CH, len - done);
-        if (used[b]) e = cudaEventSynchronize(ev[b]);                   // staging buffer free again?
-        if (e == cudaSuccess && fread(pin[b], 1, n, src.f) != n) e = cudaErrorUnknown;
-        if (e == cudaSuccess) e = cudaMemcpyAsync((uint8_t*)dst + done, pin[b], n, cudaMemcpyHostToDevice, c->stream);
-        if (e == cudaSuccess) { cudaEventRecord(ev[b], c->stream); used[b] = true; }
-        done += n; b ^= 1;
-    }
-    cudaStreamSynchronize(c->stream);
-    cudaEventDestroy(ev[0]); cudaEventDestroy(ev[1]); cudaFreeHost(pin[0]); cudaFreeHost(pin[1]);
-    return e;
-}
-
-static int groth16_load_impl(sb_ctx* c, ZkeySource& src, int shard, int n_shards, uint64_t* handle) {
-    if (!c || (!src.z && !src.f) || !handle || n_shards < 1 || shard < 0 || shard >= n_shards) return SB_ERR_ARG;
+static int groth16_load_impl(sb_ctx* c, const uint8_t* zkey, uint64_t zlen, int shard, int n_shards, uint64_t* handle) {
+    if (!c || !zkey || !handle || n_shards < 1 || shard < 0 || shard >= n_shards) return SB_ERR_ARG;
     cudaSetDevice(c->device);
-    std::map<uint32_t, Section> secs;
-    int rc = zkey_section_table(c, src, secs); if (rc) return rc;
-    for (uint32_t id : {1u, 2u, 4u, 5u, 6u, 7u, 8u, 9u}) if (!secs[id].present) return fail(c, SB_ERR_FORMAT, "Missing section " + std::to_string(id));
-    const uint8_t* s1 = zkey_host_section(src, secs, 1, 0);
-    if (!s1 || secs[1].len < 4) return fail(c, SB_ERR_FORMAT, "zkey: short read");
-    uint32_t proto; memcpy(&proto, s1, 4);
-    if (proto != 1) return fail(c, SB_ERR_FORMAT, "zkey file is not groth16");
-    const uint8_t* h = zkey_host_section(src, secs, 2, 1); uint64_t hl = secs[2].len;
-    if (!h) return fail(c, SB_ERR_FORMAT, "zkey: short read");
-    const uint32_t n8q = c->n8q, n8r = 32;
-    const uint64_t need = 4 + n8q + 4 + n8r + 12 + 3 * 2 * n8q + 3 * 4 * n8q;
-    if (hl < need) return fail(c, SB_ERR_FORMAT, "zkey header too short");
-    uint32_t v; memcpy(&v, h, 4);
-    if (v != n8q || !modulus_matches(h + 4, n8q, c->curve, false)) return fail(c, SB_ERR_FORMAT, "zkey curve does not match the context curve");
-    memcpy(&v, h + 4 + n8q, 4);
-    if (v != n8r || !modulus_matches(h + 8 + n8q, n8r, c->curve, true)) return fail(c, SB_ERR_FORMAT, "zkey curve does not match the context curve");
+    Groth16Zkey z; std::string err;
+    if (groth16_parse_zkey(zkey, zlen, z, err)) return fail(c, SB_ERR_FORMAT, err);
+    if (z.n8q != c->n8q || !modulus_matches(z.q, z.n8q, c->curve, false) || !modulus_matches(z.r, z.n8r, c->curve, true))
+        return fail(c, SB_ERR_FORMAT, "zkey curve does not match the context curve");
+    if (z.power > c->fr_s) return fail(c, SB_ERR_FORMAT, "Circuit too big for this curve");
     Groth16Key* k = new Groth16Key();
-    const uint8_t* q = h + 8 + n8q + n8r;
-    memcpy(&k->nVars, q, 4); memcpy(&k->nPublic, q + 4, 4); memcpy(&k->domainSize, q + 8, 4); q += 12;
-    const uint32_t sG1 = 2 * n8q, sG2 = 4 * n8q;
-    k->alpha1.assign(q, q + sG1); q += sG1; k->beta1.assign(q, q + sG1); q += sG1;
-    k->beta2.assign(q, q + sG2); q += sG2; k->gamma2.assign(q, q + sG2); q += sG2;
-    k->delta1.assign(q, q + sG1); q += sG1; k->delta2.assign(q, q + sG2);
-    const uint64_t n = k->domainSize, nv = k->nVars;
-    if (n == 0 || (n & (n - 1))) { delete k; return fail(c, SB_ERR_FORMAT, "domain size is not a power of two"); }
-    while (((uint64_t)1 << k->power) < n) k->power++;
-    if (k->power > c->fr_s) { delete k; return fail(c, SB_ERR_FORMAT, "Circuit too big for this curve"); }
-    if (nv < (uint64_t)k->nPublic + 1) { delete k; return fail(c, SB_ERR_FORMAT, "invalid zkey header"); }
-    if (secs[5].len != nv * sG1 || secs[6].len != nv * sG1 || secs[7].len != nv * sG2 ||
-        secs[8].len != (nv - k->nPublic - 1) * sG1 || secs[9].len != n * sG1) { delete k; return fail(c, SB_ERR_FORMAT, "zkey section size mismatch"); }
-    // coefficient section -> CSR over rows (matrix m, constraint c): src/zkey_utils.js:110-118, groth16_prove.js:147-187
-    const uint8_t* s4 = zkey_host_section(src, secs, 4, 2);
-    if (!s4 || secs[4].len < 4) { delete k; return fail(c, SB_ERR_FORMAT, "zkey: short read"); }
-    uint32_t ncoef; memcpy(&ncoef, s4, 4);
-    const uint64_t sCoef = 12 + n8r;
-    if (secs[4].len != 4 + ncoef * sCoef) { delete k; return fail(c, SB_ERR_FORMAT, "zkey coefficient section size mismatch"); }
-    const uint8_t* cf = s4 + 4;
-    std::vector<uint64_t> rowptr(2 * n + 1, 0);
-    for (uint64_t i = 0; i < ncoef; i++) {
-        uint32_t m, cc, s; memcpy(&m, cf + i * sCoef, 4); memcpy(&cc, cf + i * sCoef + 4, 4); memcpy(&s, cf + i * sCoef + 8, 4);
-        if (m > 1 || cc >= n || s >= nv) { delete k; return fail(c, SB_ERR_FORMAT, "zkey coefficient out of range"); }
-        rowptr[m * n + cc + 1]++;
-    }
-    for (uint64_t i = 0; i < 2 * n; i++) rowptr[i + 1] += rowptr[i];
-    std::vector<uint64_t> cursor(rowptr.begin(), rowptr.end() - 1);
-    std::vector<uint32_t> sig(ncoef ? ncoef : 1); std::vector<uint8_t> coef((size_t)(ncoef ? ncoef : 1) * 32);
-    for (uint64_t i = 0; i < ncoef; i++) {
-        uint32_t m, cc, s; memcpy(&m, cf + i * sCoef, 4); memcpy(&cc, cf + i * sCoef + 4, 4); memcpy(&s, cf + i * sCoef + 8, 4);
-        uint64_t p = cursor[m * n + cc]++;
-        sig[p] = s; memcpy(&coef[p * 32], cf + i * sCoef + 12, 32);
-    }
-    k->nCoef = ncoef;
-    cudaError_t e = cudaSuccess;
-    auto up = [&](void** d, const void* src, size_t bytes, size_t alloc) {
-        if (e != cudaSuccess) return;
-        e = cudaMalloc(d, alloc ? alloc : 16); if (e != cudaSuccess) return;
-        if (bytes) e = cudaMemcpy(*d, src, bytes, cudaMemcpyHostToDevice);
-    };
+    k->nVars = z.nVars; k->nPublic = z.nPublic; k->domainSize = z.domainSize; k->power = z.power; k->nCoef = z.sig.size();
+    const uint32_t sG1 = 2 * c->n8q, sG2 = 4 * c->n8q;
+    k->alpha1.assign(z.alpha1, z.alpha1 + sG1); k->beta1.assign(z.beta1, z.beta1 + sG1); k->beta2.assign(z.beta2, z.beta2 + sG2);
+    k->gamma2.assign(z.gamma2, z.gamma2 + sG2); k->delta1.assign(z.delta1, z.delta1 + sG1); k->delta2.assign(z.delta2, z.delta2 + sG2);
+    const uint64_t n = z.domainSize, nv = z.nVars;
     k->shard = shard; k->n_shards = n_shards;
     sb_shard_range(nv, shard, n_shards, &k->wlo, &k->wcnt);
     sb_shard_range(n, shard, n_shards, &k->hlo, &k->hcnt);
     const uint64_t wlo = k->wlo, wcnt = k->wcnt, hlo = k->hlo, hcnt = k->hcnt;
-    auto upsec = [&](void** d, uint32_t id, uint64_t off, uint64_t len) {
-        if (e != cudaSuccess) return;
-        e = cudaMalloc(d, len ? len : 16); if (e != cudaSuccess) return;
-        e = zkey_to_device(c, src, secs, id, off, len, *d);
-    };
-    upsec(&k->dA, 5, wlo * sG1, wcnt * sG1);
-    upsec(&k->dB1, 6, wlo * sG1, wcnt * sG1);
-    upsec(&k->dB2, 7, wlo * sG2, wcnt * sG2);
+    cudaError_t e = cudaSuccess;
+    auto alloc = [&](void** d, size_t bytes) { if (e == cudaSuccess) e = cudaMalloc(d, bytes ? bytes : 16); };
+    auto up = [&](void** d, const void* src, size_t bytes) { alloc(d, bytes); if (e == cudaSuccess) e = h2d(c, *d, src, bytes); };
+    up(&k->dA, z.A.p + wlo * sG1, wcnt * sG1);
+    up(&k->dB1, z.B1.p + wlo * sG1, wcnt * sG1);
+    up(&k->dB2, z.B2.p + wlo * sG2, wcnt * sG2);
     // C bases are indexed by signal - (nPublic+1): pad so that one sorted digit list of the witness serves A, B1, B2 and C
-    if (e == cudaSuccess) {
-        const uint64_t np1 = (uint64_t)k->nPublic + 1;
-        e = cudaMalloc(&k->dC, wcnt ? wcnt * sG1 : 16);
-        if (e == cudaSuccess && wcnt) e = cudaMemset(k->dC, 0, wcnt * sG1);
-        const uint64_t g0 = std::max(wlo, np1), g1 = wlo + wcnt;
-        if (e == cudaSuccess && g1 > g0) e = zkey_to_device(c, src, secs, 8, (g0 - np1) * sG1, (g1 - g0) * sG1, (uint8_t*)k->dC + (g0 - wlo) * sG1);
-    }
-    upsec(&k->dH, 9, hlo * sG1, hcnt * sG1);
-    up((void**)&k->d_rowptr, rowptr.data(), rowptr.size() * 8, rowptr.size() * 8);
-    up((void**)&k->d_sig, sig.data(), (size_t)ncoef * 4, (size_t)ncoef * 4);
-    up(&k->d_coef, coef.data(), (size_t)ncoef * 32, (size_t)ncoef * 32);
-    up(&k->dW, nullptr, 0, (nv + 64) * 32);   // + room for the padded slices of the distributed witness all-gather
-    up(&k->dA_T, nullptr, 0, n * 32); up(&k->dB_T, nullptr, 0, n * 32); up(&k->dC_T, nullptr, 0, n * 32); up(&k->dTmp, nullptr, 0, n * 32);
-    up(&k->dTmp2, nullptr, 0, n * 32); up(&k->dTmp3, nullptr, 0, n * 32);
-    up(&k->dWsum, nullptr, 0, 8 * 80 * 4 * 96);
+    alloc(&k->dC, wcnt * sG1);
+    if (e == cudaSuccess && wcnt) e = cudaMemsetAsync(k->dC, 0, wcnt * sG1, c->stream);
+    const uint64_t np1 = (uint64_t)k->nPublic + 1, g0 = std::max(wlo, np1), g1 = wlo + wcnt;
+    if (e == cudaSuccess && g1 > g0) e = h2d(c, (uint8_t*)k->dC + (g0 - wlo) * sG1, z.C.p + (g0 - np1) * sG1, (g1 - g0) * sG1);
+    up(&k->dH, z.H.p + hlo * sG1, hcnt * sG1);
+    up((void**)&k->d_rowptr, z.rowptr.data(), z.rowptr.size() * 8);
+    up((void**)&k->d_sig, z.sig.data(), z.sig.size() * 4);
+    up(&k->d_coef, z.coef.data(), z.coef.size());
+    alloc(&k->dW, (nv + 64) * 32);   // + room for the padded slices of the distributed witness all-gather
+    for (void** d : {&k->dA_T, &k->dB_T, &k->dC_T, &k->dTmp, &k->dTmp2, &k->dTmp3}) alloc(d, n * 32);
+    alloc(&k->dWsum, 8 * 80 * 4 * 96);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);   // the CSR vectors and the caller's bytes go away on return
     if (e != cudaSuccess) { free_key(k); return cuda_fail(c, e, "sb_groth16_load upload"); }
     if (want_precomp(c, wcnt) && want_precomp(c, hcnt)) {
         int rc2 = build_table(c, c->g1, k->dA, wcnt, &k->tA, &k->gpW);
@@ -1030,23 +889,10 @@ static int groth16_load_impl(sb_ctx* c, ZkeySource& src, int shard, int n_shards
 }
 
 int sb_groth16_load(sb_ctx* c, const uint8_t* z, uint64_t zlen, uint64_t* handle) { SB_LOCK(c);
-    if (!z) return SB_ERR_ARG;
-    ZkeySource src; src.z = z; src.zlen = zlen; return groth16_load_impl(c, src, 0, 1, handle);
+    return groth16_load_impl(c, z, zlen, 0, 1, handle);
 }
 int sb_groth16_load_sharded(sb_ctx* c, const uint8_t* z, uint64_t zlen, int shard, int n_shards, uint64_t* handle) { SB_LOCK(c);
-    if (!z) return SB_ERR_ARG;
-    ZkeySource src; src.z = z; src.zlen = zlen; return groth16_load_impl(c, src, shard, n_shards, handle);
-}
-
-int sb_groth16_load_file(sb_ctx* c, const char* path, uint64_t* handle) { SB_LOCK(c);
-    if (!c || !path) return SB_ERR_ARG;
-    cudaSetDevice(c->device);
-    FILE* f = fopen(path, "rb");
-    if (!f) return fail(c, SB_ERR_FORMAT, std::string("cannot open ") + path);
-    ZkeySource src; src.f = f;
-    int rc = groth16_load_impl(c, src, 0, 1, handle);
-    fclose(f);
-    return rc;
+    return groth16_load_impl(c, z, zlen, shard, n_shards, handle);
 }
 
 static Groth16Key* get_key(sb_ctx* c, uint64_t h) { return (c && h >= 1 && h <= c->keys.size()) ? c->keys[h - 1] : nullptr; }
@@ -1614,17 +1460,10 @@ void sb_shard_range(uint64_t total, int shard, int n_shards, uint64_t* first, ui
 
 int sb_groth16_prove_wtns(sb_ctx* c, uint64_t h, const uint8_t* w, uint64_t wlen, const uint8_t r[32], const uint8_t s[32], uint8_t* proof) { SB_LOCK(c);
     Groth16Key* k = get_key(c, h); if (!k) return fail(c, SB_ERR_ARG, "invalid groth16 handle");
-    std::map<uint32_t, Section> secs;
-    int rc = parse_binfile(c, w, wlen, "wtns", 2, secs); if (rc) return rc;
-    if (!secs[1].present || !secs[2].present) return fail(c, SB_ERR_FORMAT, "Missing section");
-    const uint8_t* hd = w + secs[1].pos;
-    if (secs[1].len < 4) return fail(c, SB_ERR_FORMAT, "wtns header too short");
-    uint32_t n8; memcpy(&n8, hd, 4);
-    if (secs[1].len < 8 + (uint64_t)n8) return fail(c, SB_ERR_FORMAT, "wtns header too short");
-    if (!modulus_matches(hd + 4, n8, c->curve, true)) return fail(c, SB_ERR_ARG, "Curve of the witness does not match the curve of the proving key");
-    uint32_t nw; memcpy(&nw, hd + 4 + n8, 4);
-    if (secs[2].len != (uint64_t)nw * n8) return fail(c, SB_ERR_FORMAT, "Invalid witness section size");
-    return sb_groth16_prove(c, h, w + secs[2].pos, nw, r, s, proof);
+    Wtns wt; std::string err;
+    if (wtns_parse(w, wlen, wt, err)) return fail(c, SB_ERR_FORMAT, err);
+    if (!modulus_matches(wt.q, wt.n8, c->curve, true)) return fail(c, SB_ERR_ARG, "Curve of the witness does not match the curve of the proving key");
+    return sb_groth16_prove(c, h, wt.values.p, wt.nWitness, r, s, proof);
 }
 
 }  // extern "C"
@@ -1657,6 +1496,7 @@ static int load_mapped(sb_ctx* c, const char* path, uint64_t* handle, int (*load
     munmap(p, (size_t)st.st_size);
     return rc;
 }
+int sb_groth16_load_file(sb_ctx* c, const char* path, uint64_t* handle) { SB_LOCK(c); return load_mapped(c, path, handle, sb_groth16_load); }
 int sb_plonk_load_file(sb_ctx* c, const char* path, uint64_t* handle) { SB_LOCK(c); return load_mapped(c, path, handle, sb_plonk_load); }
 static PlonkKeyDev* get_plonk_key(sb_ctx* c, uint64_t h) { return (c && h >= 1 && h <= c->plonk_keys.size()) ? c->plonk_keys[h - 1] : nullptr; }
 int sb_plonk_info(sb_ctx* c, uint64_t h, uint32_t* n_vars, uint32_t* n_public, uint32_t* domain_size, uint32_t* n_additions) { SB_LOCK(c);

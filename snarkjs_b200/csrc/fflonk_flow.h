@@ -7,65 +7,13 @@
 
 namespace sb {
 
-// ------------------------------------------------------------------------------------------------ zkey (fflonk) layout
-// header: src/zkey_utils.js:301-339; sections: src/fflonk_constants.js:27-44
-struct FflonkZkey {
-    uint32_t n8q = 0, n8r = 0, nVars = 0, nPublic = 0, n = 0, nAdditions = 0, nConstraints = 0; int power = 0;
-    const uint8_t *q = nullptr, *r = nullptr, *k1 = nullptr, *k2 = nullptr, *w3 = nullptr, *w4 = nullptr, *w8 = nullptr, *wr = nullptr, *X_2 = nullptr, *C0 = nullptr;
-    PlonkZkey::Sec sec[20];
-};
-inline int fflonk_parse_zkey(const uint8_t* d, uint64_t len, FflonkZkey& z, std::string& err) {
-    if (len < 12 || memcmp(d, "zkey", 4) != 0) { err = "zkey: Invalid File format"; return -1; }
-    uint32_t ver, nsec; memcpy(&ver, d + 4, 4); memcpy(&nsec, d + 8, 4);
-    if (ver > 2) { err = "Version not supported"; return -1; }
-    uint64_t pos = 12;
-    for (uint32_t i = 0; i < nsec; i++) {
-        if (pos + 12 > len) { err = "Invalid file size"; return -1; }
-        uint32_t id; uint64_t sl; memcpy(&id, d + pos, 4); memcpy(&sl, d + pos + 4, 8); pos += 12;
-        if (sl > len || pos + sl > len) { err = "Invalid file size"; return -1; }
-        if (id < 20) { if (z.sec[id].p) { err = "Section Duplicated " + std::to_string(id); return -1; } z.sec[id].p = d + pos; z.sec[id].len = sl; }
-        pos += sl;
-    }
-    if (!z.sec[1].p || z.sec[1].len < 4 || !z.sec[2].p) { err = "zkey: missing header"; return -1; }
-    uint32_t proto; memcpy(&proto, z.sec[1].p, 4);
-    if (proto != 10) { err = "zkey file is not fflonk"; return -1; }                                // fflonk_prove.js:71-73
-    const uint8_t* h = z.sec[2].p; const uint64_t hl = z.sec[2].len;
-    if (hl < 8) { err = "zkey: short header"; return -1; }
-    memcpy(&z.n8q, h, 4);
-    if (z.n8q != 32 && z.n8q != 48) { err = "zkey: unsupported base field size"; return -1; }
-    z.q = h + 4;
-    if (hl < 8 + (uint64_t)z.n8q) { err = "zkey: short header"; return -1; }
-    memcpy(&z.n8r, h + 4 + z.n8q, 4);
-    if (z.n8r != 32) { err = "zkey: unsupported scalar field size"; return -1; }
-    z.r = h + 8 + z.n8q;
-    uint64_t o = 8 + (uint64_t)z.n8q + z.n8r;
-    if (hl < o + 20 + 6 * 32 + 6 * (uint64_t)z.n8q) { err = "zkey: short header"; return -1; }
-    memcpy(&z.nVars, h + o, 4); memcpy(&z.nPublic, h + o + 4, 4); memcpy(&z.n, h + o + 8, 4); memcpy(&z.nAdditions, h + o + 12, 4); memcpy(&z.nConstraints, h + o + 16, 4);
-    o += 20;
-    z.k1 = h + o; z.k2 = h + o + 32; z.w3 = h + o + 64; z.w4 = h + o + 96; z.w8 = h + o + 128; z.wr = h + o + 160; o += 192;
-    z.X_2 = h + o; o += 4 * (uint64_t)z.n8q;
-    z.C0 = h + o;
-    if (z.n < 8 || (z.n & (z.n - 1))) { err = "zkey: domain size is not a power of two"; return -1; }
-    z.power = 0; while ((1u << z.power) < z.n) z.power++;
-    if (z.nAdditions > z.nVars || z.nConstraints + 2 > z.n || z.nPublic > z.nConstraints ||
-        (uint64_t)z.nPublic + 1 > (uint64_t)z.nVars - z.nAdditions)   /* the public signals are witness[1..nPublic] */ { err = "zkey: inconsistent header"; return -1; }
-    const uint64_t sd = (uint64_t)z.n * 32, npl = z.nPublic > 1 ? z.nPublic : 1;
-    const uint64_t want[18] = {0, 0, 0, (uint64_t)z.nAdditions * 72, (uint64_t)z.nConstraints * 4, (uint64_t)z.nConstraints * 4, (uint64_t)z.nConstraints * 4,
-                               5 * sd, 5 * sd, 5 * sd, 5 * sd, 5 * sd, 5 * sd, 5 * sd, 5 * sd, npl * 5 * sd, (9 * (uint64_t)z.n + 18) * 2 * z.n8q, 8 * sd};
-    for (int id = 3; id <= 17; id++) {
-        if (!z.sec[id].p && want[id]) { err = "zkey: missing section " + std::to_string(id); return -1; }
-        if (z.sec[id].len < want[id]) { err = "zkey: section " + std::to_string(id) + " too short"; return -1; }
-    }
-    return 0;
-}
-
-// section 17 == CPolynomial(8)(QL, QR, QO, QM, QC, S1, S2, S3) (src/fflonk_setup.js:441-464)?  One pass over the 8n coefficients.
+// C0 == CPolynomial(8)(QL, QR, QO, QM, QC, S1, S2, S3) (src/fflonk_setup.js:441-464)?  One pass over the 8n coefficients.
 inline bool fflonk_c0_is_interleave(const FflonkZkey& z) {
-    const int src[8] = {7, 8, 10, 9, 11, 12, 13, 14};       // sections of QL QR QO QM QC S1 S2 S3 (coefficients first)
-    const uint8_t* c0 = z.sec[17].p;
+    const PlonkLayout& lay = z.lay;
+    const Span* src[8] = {&lay.q_coef[0], &lay.q_coef[1], &lay.q_coef[3], &lay.q_coef[2], &lay.q_coef[4], &lay.s_coef[0], &lay.s_coef[1], &lay.s_coef[2]};
     for (uint64_t i = 0; i < z.n; i++)
         for (int j = 0; j < 8; j++)
-            if (memcmp(c0 + (8 * i + j) * 32, z.sec[src[j]].p + 32 * i, 32) != 0) return false;
+            if (memcmp(lay.c0.p + (8 * i + j) * 32, src[j]->p + 32 * i, 32) != 0) return false;
     return true;
 }
 

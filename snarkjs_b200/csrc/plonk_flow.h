@@ -13,6 +13,7 @@
 #include <string>
 #include <vector>
 #include "plonk.cuh"
+#include "zkey.h"
 
 namespace sb {
 
@@ -85,61 +86,6 @@ template <class PQ, class PR> struct PlonkTranscript {
     }
 };
 
-
-// ------------------------------------------------------------------------------------------------ zkey (plonk) layout
-// binfile container (@iden3/binfileutils readBinFile, build/snarkjs.js:17468-17498), header section 2
-// (src/zkey_utils.js:261-299), sections 3-14 (src/plonk_constants.js:1-15, written by src/plonk_setup.js:99-480)
-struct PlonkZkey {
-    uint32_t n8q = 0, n8r = 0, nVars = 0, nPublic = 0, n = 0, nAdditions = 0, nConstraints = 0; int power = 0;
-    const uint8_t *q = nullptr, *r = nullptr, *k1 = nullptr, *k2 = nullptr, *hdr_pts = nullptr, *X_2 = nullptr;
-    struct Sec { const uint8_t* p = nullptr; uint64_t len = 0; } sec[16];
-};
-inline int plonk_parse_zkey(const uint8_t* d, uint64_t len, PlonkZkey& z, std::string& err) {
-    if (len < 12 || memcmp(d, "zkey", 4) != 0) { err = "zkey: Invalid File format"; return -1; }
-    uint32_t ver, nsec; memcpy(&ver, d + 4, 4); memcpy(&nsec, d + 8, 4);
-    if (ver > 2) { err = "Version not supported"; return -1; }
-    uint64_t pos = 12;
-    for (uint32_t i = 0; i < nsec; i++) {
-        if (pos + 12 > len) { err = "Invalid file size"; return -1; }
-        uint32_t id; uint64_t sl; memcpy(&id, d + pos, 4); memcpy(&sl, d + pos + 4, 8); pos += 12;
-        if (sl > len || pos + sl > len) { err = "Invalid file size"; return -1; }
-        if (id < 16) { if (z.sec[id].p) { err = "Section Duplicated " + std::to_string(id); return -1; } z.sec[id].p = d + pos; z.sec[id].len = sl; }
-        pos += sl;
-    }
-    if (!z.sec[1].p || z.sec[1].len < 4 || !z.sec[2].p) { err = "zkey: missing header"; return -1; }
-    uint32_t proto; memcpy(&proto, z.sec[1].p, 4);
-    if (proto != 2) { err = "zkey file is not plonk"; return -1; }                                  // plonk_prove.js:58-60
-    const uint8_t* h = z.sec[2].p; const uint64_t hl = z.sec[2].len;
-    if (hl < 8) { err = "zkey: short header"; return -1; }
-    memcpy(&z.n8q, h, 4);
-    if (z.n8q != 32 && z.n8q != 48) { err = "zkey: unsupported base field size"; return -1; }
-    z.q = h + 4;
-    if (hl < 8 + (uint64_t)z.n8q) { err = "zkey: short header"; return -1; }
-    memcpy(&z.n8r, h + 4 + z.n8q, 4);
-    if (z.n8r != 32) { err = "zkey: unsupported scalar field size"; return -1; }
-    z.r = h + 8 + z.n8q;
-    uint64_t o = 8 + (uint64_t)z.n8q + z.n8r;
-    if (hl < o + 20 + 2 * 32 + 8 * 2 * (uint64_t)z.n8q + 4 * (uint64_t)z.n8q) { err = "zkey: short header"; return -1; }
-    memcpy(&z.nVars, h + o, 4); memcpy(&z.nPublic, h + o + 4, 4); memcpy(&z.n, h + o + 8, 4); memcpy(&z.nAdditions, h + o + 12, 4); memcpy(&z.nConstraints, h + o + 16, 4);
-    o += 20;
-    z.k1 = h + o; z.k2 = h + o + 32; o += 64;
-    z.hdr_pts = h + o; o += 8 * 2 * (uint64_t)z.n8q;
-    z.X_2 = h + o;
-    if (z.n < 8 || (z.n & (z.n - 1))) { err = "zkey: domain size is not a power of two"; return -1; }
-    z.power = 0; while ((1u << z.power) < z.n) z.power++;
-    if (z.nAdditions > z.nVars || z.nConstraints > z.n || z.nPublic > z.nConstraints ||
-        (uint64_t)z.nPublic + 1 > (uint64_t)z.nVars - z.nAdditions)   /* the public signals are witness[1..nPublic] */ { err = "zkey: inconsistent header"; return -1; }
-    const uint64_t sd = (uint64_t)z.n * 32, npl = z.nPublic > 1 ? z.nPublic : 1;
-    const uint64_t want[15] = {0, 0, 0, (uint64_t)z.nAdditions * 72, (uint64_t)z.nConstraints * 4, (uint64_t)z.nConstraints * 4, (uint64_t)z.nConstraints * 4,
-                               5 * sd, 5 * sd, 5 * sd, 5 * sd, 5 * sd, 15 * sd, npl * 5 * sd, ((uint64_t)z.n + 6) * 2 * z.n8q};
-    for (int id = 3; id <= 14; id++) {
-        if (!z.sec[id].p && want[id]) { err = "zkey: missing section " + std::to_string(id); return -1; }
-        // the reference writes max(nPublic, 1) Lagrange polynomials; accept exactly nPublic as well
-        uint64_t need = id == 13 ? (uint64_t)z.nPublic * 5 * sd : want[id];
-        if (z.sec[id].len < need) { err = "zkey: section " + std::to_string(id) + " too short"; return -1; }
-    }
-    return 0;
-}
 
 template <class F> inline F fr_from_u64(uint64_t x) { F a = F::zero(); a.v[0] = (uint32_t)x; a.v[1] = (uint32_t)(x >> 32); return F::to_mont(a); }
 template <class F> inline F fr_pow2k(F x, int k) { for (int i = 0; i < k; i++) x = F::sqr(x); return x; }   // x^(2^k)

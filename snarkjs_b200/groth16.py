@@ -72,29 +72,6 @@ def read_zkey_header_groth16(data: bytes):
     return z
 
 
-def read_zkey_header_groth16_prefix(head: bytes):
-    """Header fields from the first bytes of a zkey whose sections 1 and 2 come first (only q / r are needed here)."""
-    if head[:4] != b"zkey":
-        raise SbError("zkey: Invalid File format")
-    pos = 12
-    found = {}
-    while pos + 12 <= len(head) and len(found) < 2:
-        sid, ln = struct.unpack_from("<IQ", head, pos)
-        pos += 12
-        if sid in (1, 2) and pos + ln <= len(head):
-            found[sid] = head[pos:pos + ln]
-        pos += ln
-    if 2 not in found:
-        raise SbError("header not in prefix")
-    h = found[2]
-    n8q = struct.unpack_from("<I", h, 0)[0]
-    q = int.from_bytes(h[4:4 + n8q], "little")
-    n8r = struct.unpack_from("<I", h, 4 + n8q)[0]
-    r = int.from_bytes(h[8 + n8q:8 + n8q + n8r], "little")
-    nVars, nPublic, domainSize = struct.unpack_from("<III", h, 8 + n8q + n8r)
-    return {"n8q": n8q, "q": q, "n8r": n8r, "r": r, "nVars": nVars, "nPublic": nPublic, "domainSize": domainSize}
-
-
 def random_fr(curve: Curve) -> bytes:
     """Fr.random(): a uniform value below r, used directly as the Montgomery representation (13019-13035)."""
     nbytes = 32
@@ -144,22 +121,16 @@ class ProvingKey:
 
     @classmethod
     def from_file(cls, path: str, curve: Curve):
-        """Streams the .zkey from disk (sb_groth16_load_file): base sections go to HBM through pinned double buffers."""
+        """Loads the key from disk (sb_groth16_load_file: mapped read-only, streamed to HBM section by section)."""
         self = cls.__new__(cls)
         self.curve, self._own_curve = curve, False
         h = ctypes.c_uint64()
         curve.check(curve.lib.sb_groth16_load_file(curve.handle, path.encode(), ctypes.byref(h)))   # validates the container
         self.handle = h.value
-        with open(path, "rb") as f:
-            head = f.read(1 << 16)
-        # header only (sections 1-2 are at the front in files written by snarkjs; fall back to a full read otherwise)
-        try:
-            self.header = read_zkey_header_groth16_prefix(head)
-        except Exception:
-            self.header = read_zkey_header_groth16(open(path, "rb").read())
         nv, npub, ds = ctypes.c_uint32(), ctypes.c_uint32(), ctypes.c_uint32()
         curve.check(curve.lib.sb_groth16_info(curve.handle, self.handle, ctypes.byref(nv), ctypes.byref(npub), ctypes.byref(ds)))
         self.nVars, self.nPublic, self.domainSize = nv.value, npub.value, ds.value
+        self.header = {"n8q": curve.n8q, "q": curve.q, "n8r": 32, "r": curve.r, "nVars": nv.value, "nPublic": npub.value, "domainSize": ds.value}
         return self
 
     def prove_raw(self, witness, r: bytes, s: bytes) -> bytes:

@@ -101,3 +101,23 @@ template <class F> struct HostBackend {
     }
 };
 
+// The key arrays of a parsed PLONK / fflonk key (zkey.h's PlonkLayout), copied out of the container the way the device
+// loaders upload them, with the view's pointers set to them
+template <class F> struct HostKeyArrays {
+    std::vector<uint32_t> sig, order, maps[3];
+    std::vector<F> fac, q_coef[5], q_ev[5], s_coef[3], s_ev[3], lag;
+    static const F* copy(std::vector<F>& v, const Span& s) { v.resize(s.len / sizeof(F)); if (s.len) memcpy(v.data(), s.p, s.len); return v.data(); }
+    template <class View> void fill(const PlonkHeader& z, const PlonkLayout& lay, View& k) {
+        const uint64_t n = z.n;
+        sig.assign(2 * (size_t)z.nAdditions + 2, 0); fac.assign(2 * (size_t)z.nAdditions + 2, F::zero());
+        for (uint32_t i = 0; i < z.nAdditions; i++) { memcpy(&sig[2 * i], lay.additions.p + 72 * (size_t)i, 8); memcpy(&fac[2 * i], lay.additions.p + 72 * (size_t)i + 8, 64); }
+        plonk_addition_levels(sig.data(), z.nAdditions, z.nVars - z.nAdditions, order, k.level_end);
+        k.add_sig = sig.data(); k.add_fac = fac.data(); k.add_order = order.data();
+        for (int j = 0; j < 3; j++) { maps[j].assign(z.nConstraints + 1, 0); if (lay.maps[j].len) memcpy(maps[j].data(), lay.maps[j].p, lay.maps[j].len); k.map[j] = maps[j].data(); }
+        for (int j = 0; j < 5; j++) { k.q_coef[j] = copy(q_coef[j], lay.q_coef[j]); k.q_ev[j] = copy(q_ev[j], lay.q_ev[j]); }
+        for (int j = 0; j < 3; j++) { k.s_coef[j] = copy(s_coef[j], lay.s_coef[j]); k.s_ev[j] = copy(s_ev[j], lay.s_ev[j]); }
+        lag.assign((size_t)(z.nPublic > 1 ? z.nPublic : 1) * 4 * n, F::zero());                // polynomials the key leaves out stay zero
+        for (size_t j = 0; j < lay.lag.size(); j++) memcpy(lag.data() + j * 4 * n, lay.lag[j].p, lay.lag[j].len);
+        k.lag = lag.data();
+    }
+};

@@ -40,27 +40,16 @@ static int prove_impl(void* so, int curve, const FflonkZkey& z, const uint8_t* w
     if (!be.fft || !be.msm || !be.gop || !root) { err = "oracle symbols missing"; return -1; }
     const uint64_t n = z.n;
     // the reference reserves 16n points and leaves zeros past 9n + 18 (fflonk_prove.js:164-169); 9n + 18 are enough here
-    be.curve = curve; be.n8q = z.n8q; be.ptau = z.sec[16].p;
+    be.curve = curve; be.n8q = z.n8q; be.ptau = z.lay.ptau.p;
     be.pow_store.reserve(256);
     FflonkKeyView<F> k;
     k.nVars = z.nVars; k.nPublic = z.nPublic; k.n = z.n; k.nAdditions = z.nAdditions; k.nConstraints = z.nConstraints; k.power = z.power;
     memcpy(&k.k1, z.k1, 32); memcpy(&k.k2, z.k2, 32); memcpy(&k.w3, z.w3, 32); memcpy(&k.w4, z.w4, 32); memcpy(&k.w8, z.w8, 32); memcpy(&k.wr, z.wr, 32);
     F w2n, w4n; root(curve, z.power, (uint8_t*)&k.wn); root(curve, z.power + 1, (uint8_t*)&w2n); root(curve, z.power + 2, (uint8_t*)&w4n);
     k.c0_point = z.C0; k.aff_bytes = 2 * z.n8q;
-    std::vector<uint32_t> sig(2 * (size_t)z.nAdditions + 2), order; std::vector<F> fac(2 * (size_t)z.nAdditions + 2);
-    for (uint32_t i = 0; i < z.nAdditions; i++) { memcpy(&sig[2 * i], z.sec[3].p + 72 * (size_t)i, 8); memcpy(&fac[2 * i], z.sec[3].p + 72 * (size_t)i + 8, 64); }
-    plonk_addition_levels(sig.data(), z.nAdditions, z.nVars - z.nAdditions, order, k.level_end);
-    k.add_sig = sig.data(); k.add_fac = fac.data(); k.add_order = order.data();
-    std::vector<uint32_t> maps[3];
-    for (int j = 0; j < 3; j++) { maps[j].resize(z.nConstraints + 1); memcpy(maps[j].data(), z.sec[4 + j].p, 4 * (size_t)z.nConstraints); k.map[j] = maps[j].data(); }
-    std::vector<F> qc[5], qe[5], sc[3], se[3], lag, c0(8 * n);
-    for (int j = 0; j < 5; j++) { qc[j].resize(n); qe[j].resize(4 * n); memcpy(qc[j].data(), z.sec[7 + j].p, 32 * n); memcpy(qe[j].data(), z.sec[7 + j].p + 32 * n, 128 * n); k.q_coef[j] = qc[j].data(); k.q_ev[j] = qe[j].data(); }
-    for (int j = 0; j < 3; j++) { sc[j].resize(n); se[j].resize(4 * n); memcpy(sc[j].data(), z.sec[12 + j].p, 32 * n); memcpy(se[j].data(), z.sec[12 + j].p + 32 * n, 128 * n); k.s_coef[j] = sc[j].data(); k.s_ev[j] = se[j].data(); }
-    const uint32_t nl = z.nPublic > 1 ? z.nPublic : 1;
-    lag.assign((size_t)nl * 4 * n, F::zero());
-    for (uint32_t j = 0; j < nl; j++) memcpy(lag.data() + (size_t)j * 4 * n, z.sec[15].p + 160 * n * j + 32 * n, 128 * n);
-    k.lag = lag.data();
-    memcpy(c0.data(), z.sec[17].p, 256 * n); k.c0 = c0.data();
+    HostKeyArrays<F> arrays; arrays.fill(z, z.lay, k);
+    std::vector<F> c0;
+    k.c0 = HostKeyArrays<F>::copy(c0, z.lay.c0);
     k.c0_is_interleave = fflonk_c0_is_interleave(z);
     be.make_pow(k.wn, n, k.wpow, 0);
     be.make_pow(w2n, 2 * n, k.w2pow, 0);

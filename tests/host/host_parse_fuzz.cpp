@@ -1,9 +1,9 @@
-// Mutation fuzzing of the PLONK / fflonk zkey parsers and of the host-side load logic that consumes their output
-// (plonk_parse_zkey, fflonk_parse_zkey, the section reads sb_plonk_load / sb_fflonk_load perform, plonk_addition_levels),
-// built with -fsanitize=address,undefined by tests/test_host_templates.py.  Every mutated container must either be
-// rejected with a message or be accepted with every section read staying inside the buffer; the sanitizers turn an
-// out-of-bounds read or an overflowed size into a crash.  The buffer handed to the parser is an exact-size heap block,
-// so reading one byte past the file is detected.   usage: host_parse_fuzz plonk|fflonk <zkey file> <iterations>
+// Mutation fuzzing of the container parsers of zkey.h (plonk_parse_zkey, fflonk_parse_zkey, groth16_parse_zkey,
+// wtns_parse) and of the host-side load logic that consumes their output (plonk_addition_levels), built with
+// -fsanitize=address,undefined by tests/test_host_templates.py.  Every mutated container must either be rejected with a
+// message or be accepted with every span and CSR entry the parser returned staying inside the buffer; the sanitizers turn
+// an out-of-bounds read or an overflowed size into a crash.  The buffer handed to the parser is an exact-size heap block,
+// so reading one byte past the file is detected.   usage: host_parse_fuzz plonk|fflonk|groth16|wtns <file> <iterations>
 #include <cstdio>
 #include <cstdlib>
 #include <fstream>
@@ -16,29 +16,39 @@ static uint64_t rnd() { st ^= st << 13; st ^= st >> 7; st ^= st << 17; return st
 static volatile uint64_t sink;
 static void touch(const uint8_t* p, uint64_t len) { uint64_t s = 0; for (uint64_t i = 0; i < len; i += 97) s += p[i]; if (len) s += p[len - 1]; sink += s; }
 
-// what sb_plonk_load reads after a successful parse (api_plonk.inl plonk_load_impl), with host reads in place of uploads
-static void consume_plonk(const PlonkZkey& z) {
-    const uint64_t n = z.n, sd = n * 32;
-    touch(z.sec[2].p, z.sec[2].len); touch(z.q, z.n8q); touch(z.r, z.n8r); touch(z.k1, 32); touch(z.k2, 32);
-    touch(z.hdr_pts, 8 * 2 * (uint64_t)z.n8q); touch(z.X_2, 4 * (uint64_t)z.n8q);
+static void touch(const Span& s) { touch(s.p, s.len); }
+
+// every span the parser returned, with host reads in place of the loaders' uploads
+static void consume(const PlonkHeader& z, const PlonkLayout& lay) {
+    touch(z.header); touch(z.q, z.n8q); touch(z.r, z.n8r); touch(z.k1, 32); touch(z.k2, 32);
     const uint32_t na = z.nAdditions;
     std::vector<uint32_t> sig(2 * (size_t)na + 2), order, level_end;
-    for (uint32_t i = 0; i < na; i++) { memcpy(&sig[2 * (size_t)i], z.sec[3].p + 72 * (size_t)i, 8); touch(z.sec[3].p + 72 * (size_t)i + 8, 64); }
+    for (uint32_t i = 0; i < na; i++) { memcpy(&sig[2 * (size_t)i], lay.additions.p + 72 * (size_t)i, 8); touch(lay.additions.p + 72 * (size_t)i + 8, 64); }
     plonk_addition_levels(sig.data(), na, z.nVars - na, order, level_end);
     uint64_t tot = 0; for (uint32_t e : level_end) tot = e;
     if (na && tot != na) { fprintf(stderr, "addition levels do not cover all additions\n"); abort(); }
     for (uint32_t o : order) if (o >= na) { fprintf(stderr, "addition order out of range\n"); abort(); }
-    for (int j = 0; j < 3; j++) touch(z.sec[4 + j].p, (uint64_t)z.nConstraints * 4);
-    for (int j = 0; j < 5; j++) touch(z.sec[7 + j].p, 5 * sd);
-    touch(z.sec[12].p, 15 * sd);
-    const uint32_t nl = z.nPublic > 1 ? z.nPublic : 1, have = (uint32_t)(z.sec[13].len / (5 * sd));
-    for (uint32_t j = 0; j < nl && j < have; j++) touch(z.sec[13].p + 5 * sd * j + sd, 4 * sd);
-    touch(z.sec[14].p, (n + 6) * 2 * (uint64_t)z.n8q);
+    for (const Span& s : lay.maps) touch(s);
+    for (int j = 0; j < 5; j++) { touch(lay.q_coef[j]); touch(lay.q_ev[j]); }
+    for (int j = 0; j < 3; j++) { touch(lay.s_coef[j]); touch(lay.s_ev[j]); }
+    for (const Span& s : lay.lag) touch(s);
+    touch(lay.ptau); touch(lay.c0);
+}
+static void consume(const Groth16Zkey& z) {
+    touch(z.q, z.n8q); touch(z.r, z.n8r);
+    for (const uint8_t* p : {z.alpha1, z.beta1, z.delta1}) touch(p, 2 * (uint64_t)z.n8q);
+    for (const uint8_t* p : {z.beta2, z.gamma2, z.delta2}) touch(p, 4 * (uint64_t)z.n8q);
+    for (const Span& s : {z.A, z.B1, z.B2, z.C, z.H}) touch(s);
+    if (z.rowptr.size() != 2 * (uint64_t)z.domainSize + 1 || z.rowptr.back() != z.sig.size() || z.coef.size() != 32 * z.sig.size()) { fprintf(stderr, "CSR shape\n"); abort(); }
+    for (size_t i = 0; i + 1 < z.rowptr.size(); i++) if (z.rowptr[i] > z.rowptr[i + 1]) { fprintf(stderr, "CSR row pointers not monotone\n"); abort(); }
+    for (uint32_t s : z.sig) if (s >= z.nVars) { fprintf(stderr, "CSR signal out of range\n"); abort(); }
+    touch(z.coef.data(), z.coef.size());
 }
 
 int main(int argc, char** argv) {
     if (argc < 4) return 2;
-    const bool ff = std::string(argv[1]) == "fflonk";
+    const std::string proto = argv[1];
+    if (proto != "plonk" && proto != "fflonk" && proto != "groth16" && proto != "wtns") return 2;
     std::ifstream f(argv[2], std::ios::binary);
     std::vector<uint8_t> good((std::istreambuf_iterator<char>(f)), std::istreambuf_iterator<char>());
     const long iters = atol(argv[3]);
@@ -58,12 +68,17 @@ int main(int argc, char** argv) {
             if (mode == 5) { uint64_t p = 12 + rnd() % std::min<uint64_t>(len - 12, 600); memset(buf + p, rnd() % 2 ? 0xff : 0, std::min<uint64_t>(12, len - p)); }                   // a smashed section header
         }
         std::string err; int rc;
-        if (ff) { FflonkZkey z; rc = fflonk_parse_zkey(buf, len, z, err); if (!rc) { for (int id = 1; id < 20; id++) if (z.sec[id].p) touch(z.sec[id].p, z.sec[id].len); touch(z.q, z.n8q); touch(z.r, z.n8r); if (z.C0) touch(z.C0, 2 * (uint64_t)z.n8q); } }
-        else { PlonkZkey z; rc = plonk_parse_zkey(buf, len, z, err); if (!rc) consume_plonk(z); }
+        if (proto == "plonk") { PlonkZkey z; rc = plonk_parse_zkey(buf, len, z, err); if (!rc) { consume(z, z.lay); touch(z.hdr_pts, 16 * (uint64_t)z.n8q); touch(z.X_2, 4 * (uint64_t)z.n8q); } }
+        else if (proto == "fflonk") {
+            FflonkZkey z; rc = fflonk_parse_zkey(buf, len, z, err);
+            if (!rc) { consume(z, z.lay); for (const uint8_t* p : {z.w3, z.w4, z.w8, z.wr}) touch(p, 32); touch(z.X_2, 4 * (uint64_t)z.n8q); touch(z.C0, 2 * (uint64_t)z.n8q); fflonk_c0_is_interleave(z); }
+        }
+        else if (proto == "groth16") { Groth16Zkey z; rc = groth16_parse_zkey(buf, len, z, err); if (!rc) consume(z); }
+        else { Wtns w; rc = wtns_parse(buf, len, w, err); if (!rc) { touch(w.q, w.n8); touch(w.values); } }
+        free(buf);
         if (rc) { if (err.empty()) { fprintf(stderr, "rejected without a message (iteration %ld)\n", it); return 1; } rejected++; }
         else accepted++;
         if (it == 0 && rc) { fprintf(stderr, "the unmodified key was rejected: %s\n", err.c_str()); return 1; }
-        free(buf);
     }
     printf("FUZZ OK %s: %ld accepted, %ld rejected\n", argv[1], accepted, rejected);
     return 0;

@@ -10,7 +10,7 @@ static int prove_impl(void* so, int curve, const PlonkZkey& z, const uint8_t* wi
     be.fft = (or_fft_t)dlsym(so, "or_fr_fft"); be.msm = (or_msm_t)dlsym(so, "or_multiexp_affine"); be.gop = (or_gop_t)dlsym(so, "or_group_op");
     or_root_t root = (or_root_t)dlsym(so, "or_fr_root");
     if (!be.fft || !be.msm || !be.gop || !root) { err = "oracle symbols missing"; return -1; }
-    be.curve = curve; be.n8q = z.n8q; be.ptau = z.sec[14].p;
+    be.curve = curve; be.n8q = z.n8q; be.ptau = z.lay.ptau.p;
     be.pow_store.reserve(64);
     PlonkKeyView<F> k;
     k.nVars = z.nVars; k.nPublic = z.nPublic; k.n = z.n; k.nAdditions = z.nAdditions; k.nConstraints = z.nConstraints; k.power = z.power;
@@ -19,21 +19,7 @@ static int prove_impl(void* so, int curve, const PlonkZkey& z, const uint8_t* wi
     plonk_mulz_tables<F>(w2, k.z1, k.z2, k.z3);
     k.hdr_pts = z.hdr_pts; k.aff_bytes = 2 * z.n8q;
     const uint64_t n = z.n;
-    // additions: split (s1, s2, f1, f2) records into the two arrays the kernels read
-    std::vector<uint32_t> sig(2 * (size_t)z.nAdditions + 2), order; std::vector<F> fac(2 * (size_t)z.nAdditions + 2);
-    for (uint32_t i = 0; i < z.nAdditions; i++) { memcpy(&sig[2 * i], z.sec[3].p + 72 * (size_t)i, 8); memcpy(&fac[2 * i], z.sec[3].p + 72 * (size_t)i + 8, 64); }
-    plonk_addition_levels(sig.data(), z.nAdditions, z.nVars - z.nAdditions, order, k.level_end);
-    k.add_sig = sig.data(); k.add_fac = fac.data(); k.add_order = order.data();
-    std::vector<uint32_t> maps[3];
-    for (int j = 0; j < 3; j++) { maps[j].resize(z.nConstraints + 1); memcpy(maps[j].data(), z.sec[4 + j].p, 4 * (size_t)z.nConstraints); k.map[j] = maps[j].data(); }
-    std::vector<F> qc[5], qe[5], sc[3], se[3], lag;
-    for (int j = 0; j < 5; j++) { qc[j].resize(n); qe[j].resize(4 * n); memcpy(qc[j].data(), z.sec[7 + j].p, 32 * n); memcpy(qe[j].data(), z.sec[7 + j].p + 32 * n, 128 * n); k.q_coef[j] = qc[j].data(); k.q_ev[j] = qe[j].data(); }
-    for (int j = 0; j < 3; j++) { sc[j].resize(n); se[j].resize(4 * n); memcpy(sc[j].data(), z.sec[12].p + 160 * n * j, 32 * n); memcpy(se[j].data(), z.sec[12].p + 160 * n * j + 32 * n, 128 * n); k.s_coef[j] = sc[j].data(); k.s_ev[j] = se[j].data(); }
-    const uint32_t nl = z.nPublic > 1 ? z.nPublic : 1;
-    const uint32_t nl_have = (uint32_t)(z.sec[13].len / (160 * n));
-    lag.assign((size_t)nl * 4 * n, F::zero());
-    for (uint32_t j = 0; j < nl && j < nl_have; j++) memcpy(lag.data() + (size_t)j * 4 * n, z.sec[13].p + 160 * n * j + 32 * n, 128 * n);
-    k.lag = lag.data();
+    HostKeyArrays<F> arrays; arrays.fill(z, z.lay, k);
     be.make_pow(k.wn, n, k.wpow, 0);
     be.make_pow(k.w4n, 4 * n, k.w4pow, 0);
     PlonkWork<F> w;

@@ -489,8 +489,8 @@ def test_plonk_polynomial_wrappers_on_fixture_goldens(bn, golden):
 
 
 def test_groth16_streamed_zkey_file(bn, golden, tmp_path):
-    """sb_groth16_load_file: sections streamed from disk through pinned double buffers; same proof as the in-memory
-    load; malformed files are rejected with the reference's messages."""
+    """sb_groth16_load_file: the key mapped from disk and streamed through the staging buffers; same proof as the
+    in-memory load; malformed files are rejected with the reference's messages."""
     from snarkjs_b200 import groth16, SbError
     g = golden("groth16_case.npz")
     zkey, wt = g["zkey"].tobytes(), g["wtns"].tobytes()

@@ -4,6 +4,7 @@ the oracle) and compared with oracle/fflonk.py proof for proof on the reference'
 import ctypes
 import json
 import os
+import struct
 import subprocess
 
 import pytest
@@ -99,3 +100,7 @@ def test_host_fflonk_errors(hostlib, golden):
     assert rc != 0 and err.startswith("Invalid witness length. Circuit: ")
     rc, err, _ = host_prove(hostlib, bytes(golden("plonk_case.npz")["zkey"]), wtns, BLINDERS)
     assert rc != 0 and err == "zkey file is not fflonk"
+    bad = bytearray(zkey) + struct.pack("<IQ", 20, 0) * 2                 # a section id fflonk does not use, twice
+    struct.pack_into("<I", bad, 8, struct.unpack_from("<I", zkey, 8)[0] + 2)
+    rc, err, _ = host_prove(hostlib, bytes(bad), wtns, BLINDERS)
+    assert rc != 0 and err == "Section Duplicated 20"

@@ -164,6 +164,11 @@ def test_host_parser_rejects_malformed_keys(hostlib):
     struct.pack_into("<Q", bad, 16, 1 << 40)
     rc, err, _ = host_prove(hostlib, bytes(bad), wtns, BLINDERS)
     assert rc != 0 and err == "Invalid file size"
+    # a section id PLONK does not use, twice
+    bad = bytearray(zkey) + struct.pack("<IQ", 16, 0) * 2
+    struct.pack_into("<I", bad, 8, struct.unpack_from("<I", zkey, 8)[0] + 2)
+    rc, err, _ = host_prove(hostlib, bytes(bad), wtns, BLINDERS)
+    assert rc != 0 and err == "Section Duplicated 16"
     # domain size that is not a power of two (header field at a fixed offset inside section 2)
     data, secs = orc.read_binfile(zkey, "zkey", 2)
     pos = secs[2][0][0] + 4 + 32 + 4 + 32 + 8
