@@ -74,6 +74,7 @@ struct Groth16Key {
     // device work buffers
     bool witness_resident = false;   // set by the first upload: sb_groth16_prove_resident refuses to run before it
     void *dW = nullptr, *dA_T = nullptr, *dB_T = nullptr, *dC_T = nullptr, *dTmp = nullptr, *dTmp2 = nullptr, *dTmp3 = nullptr, *dWsum = nullptr;
+    size_t wsum_bytes = 0;           // size of dWsum (groth16_wsum_room grows it)
 };
 
 }  // namespace
@@ -98,7 +99,8 @@ struct sb_ctx {
     MsmScratch sort_scratch2, bscr[5];           // per-MSM scratch for the overlapped Groth16 pipeline
     cudaStream_t aux[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // high-priority side streams (tails, NTT chain)
     cudaEvent_t pev[16];                         // pipeline events
-    uint8_t* pinned = nullptr;                   // 256 KiB pinned staging (window sums, counters)
+    uint8_t* pinned = nullptr;                   // pinned staging of a Groth16 proof's window sums and counters: 256 KiB,
+    size_t pinned_bytes = 0;                     // grown by groth16_wsum_room when a geometry needs more
     uint8_t* stage[2] = {nullptr, nullptr};      // 2 x 8 MiB pinned staging for large pageable host buffers
     cudaEvent_t stage_ev[2];
     MsmLaunchStats stats;
@@ -490,6 +492,7 @@ int sb_create(int curve, int device_id, sb_ctx** out) {
     { int lo = 0, hi = 0; cudaDeviceGetStreamPriorityRange(&lo, &hi);
       for (auto& st : c->aux) cudaStreamCreateWithPriority(&st, cudaStreamDefault, hi); }
     if (cudaHostAlloc((void**)&c->pinned, 256 * 1024, cudaHostAllocDefault) != cudaSuccess) c->pinned = nullptr;
+    else c->pinned_bytes = 256 * 1024;
     for (int i = 0; i < 2; i++) { if (cudaHostAlloc((void**)&c->stage[i], STAGE_BYTES, cudaHostAllocDefault) != cudaSuccess) c->stage[i] = nullptr; cudaEventCreateWithFlags(&c->stage_ev[i], cudaEventDisableTiming); }
     init_generators(c);
     int rc = curve == SB_BN254 ? init_roots<BnFr>(c) : init_roots<BlsFr>(c);
@@ -873,6 +876,7 @@ static int groth16_load_impl(sb_ctx* c, const uint8_t* zkey, uint64_t zlen, int 
     alloc(&k->dW, (nv + 64) * 32);   // + room for the padded slices of the distributed witness all-gather
     for (void** d : {&k->dA_T, &k->dB_T, &k->dC_T, &k->dTmp, &k->dTmp2, &k->dTmp3}) alloc(d, n * 32);
     alloc(&k->dWsum, 8 * 80 * 4 * 96);
+    if (e == cudaSuccess) k->wsum_bytes = 8 * 80 * 4 * 96;
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);   // the CSR vectors and the caller's bytes go away on return
     if (e != cudaSuccess) { free_key(k); return cuda_fail(c, e, "sb_groth16_load upload"); }
     if (want_precomp(c, wcnt) && want_precomp(c, hcnt)) {
@@ -997,6 +1001,26 @@ int sb_dist_chain_owner(int chain, int world) { return world > 0 ? chain % world
 // plain (non-Montgomery) r and s: when given, the prover folds s*A + r*B1 + H into the C partial as soon as A and B1 land
 // (hidden behind the C and H MSMs), so that the proof assembly after the last MSM is three additions
 struct ProofScalars { uint8_t rp[32], sp[32]; };
+
+// The window sums of a proof's MSMs land in the key's device buffer and come back through the context's pinned area.
+// Their first sizes hold the table geometries and the plain ones over about a thousand points; a plain MSM over fewer
+// points takes narrower windows (3 bits, 86 windows, for 49 points or fewer on BN254), which need more room, so both
+// buffers grow to what the geometries of the call need.  Earlier calls have finished with them by now.
+static int groth16_wsum_room(sb_ctx* c, Groth16Key* k, size_t dev_bytes, size_t host_bytes) {
+    if (dev_bytes > k->wsum_bytes) {
+        void* old = k->dWsum; k->dWsum = nullptr; k->wsum_bytes = 0;
+        if (old) CU(c, cudaFree(old));
+        CU(c, cudaMalloc(&k->dWsum, dev_bytes));
+        k->wsum_bytes = dev_bytes;
+    }
+    if (host_bytes > c->pinned_bytes) {
+        uint8_t* old = c->pinned; c->pinned = nullptr; c->pinned_bytes = 0;
+        if (old) CU(c, cudaFreeHost(old));
+        CU(c, cudaHostAlloc((void**)&c->pinned, host_bytes, cudaHostAllocDefault));
+        c->pinned_bytes = host_bytes;
+    }
+    return 0;
+}
 
 // device part of the prover: returns the five MSM partials (A, B1, C, H | B2) as host XYZZ bytes.
 // dist: this context is rank c->rank of c->world (sb_comm_init_rank); the witness is uploaded in slices and all-gathered,
@@ -1124,7 +1148,8 @@ static int groth16_device(sb_ctx* c, Groth16Key* k, const uint8_t* witness, uint
         const bool pre = k->tA != nullptr;
         if (pre) { gw = k->gpW; gw.first = wb; gh = k->gpH; gh.first = hb; }
         const size_t w1 = (size_t)gw.wsum_points() * G1.xyzz_bytes, w2 = (size_t)gw.wsum_points() * G2.xyzz_bytes, wh = (size_t)gh.wsum_points() * G1.xyzz_bytes;
-        if (3 * w1 + w2 + wh + 64 > 256 * 1024 || 3 * w1 + w2 + wh > (size_t)8 * 80 * 4 * 96) return fail(c, SB_ERR_ARG, "window buffer too small");
+        rc = groth16_wsum_room(c, k, 3 * w1 + w2 + wh, 3 * w1 + w2 + wh + 64);
+        if (rc) return rc;
         uint8_t* dws = (uint8_t*)k->dWsum; uint8_t* hws = c->pinned;
         uint64_t* hcounts = (uint64_t*)(c->pinned + 3 * w1 + w2 + wh);
         CU(c, cudaEventRecord(c->pev[0], s0));                       // witness resident
@@ -1180,9 +1205,10 @@ static int groth16_device(sb_ctx* c, Groth16Key* k, const uint8_t* witness, uint
         MsmSorted s;
         rc = msm_sort_entries((const uint8_t*)k->dW + (wlo + off) * 32, 32, cn, g, c->sort_scratch, c->stream, &s, &c->stats);
         if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
-        uint8_t* ws = (uint8_t*)k->dWsum;
         size_t w1 = (size_t)g.wsum_points() * G1.xyzz_bytes, w2 = (size_t)g.wsum_points() * G2.xyzz_bytes;
-        if (3 * w1 + w2 > (size_t)8 * 80 * 4 * 96) return fail(c, SB_ERR_ARG, "window buffer too small");
+        rc = groth16_wsum_room(c, k, 3 * w1 + w2, 0);
+        if (rc) return rc;
+        uint8_t* ws = (uint8_t*)k->dWsum;
         c->stats.cur_tag = SB_G1;
         rc = G1.buckets((const uint8_t*)k->dA + base * G1.aff_bytes, s, c->bucket_scratch, c->stream, ws, &c->stats, nullptr, nullptr); if (rc) return cuda_fail(c, (cudaError_t)rc, "msm A");
         rc = G1.buckets((const uint8_t*)k->dB1 + base * G1.aff_bytes, s, c->bucket_scratch, c->stream, ws + w1, &c->stats, nullptr, nullptr); if (rc) return cuda_fail(c, (cudaError_t)rc, "msm B1");
