@@ -61,6 +61,11 @@ int sb_msm_registered(sb_ctx* ctx, uint64_t handle, uint64_t first, const uint8_
 /* Same, additionally returning the un-normalised extended-Jacobian partial (X,Y,ZZ,ZZZ; 4 or 8 coordinates) that
  * sb_msm_sum_partials combines — the exchange unit of the multi-GPU MSM (one rank per GPU, SURVEY.md §8e). */
 int sb_msm_registered_partial(sb_ctx* ctx, uint64_t handle, uint64_t first, const uint8_t* scalars, uint32_t scalar_bytes, uint64_t n, uint8_t* partial_out);
+/* count MSMs over the same registered bases [first, first+n): scalars = count * n * scalar_bytes; out = count normalised Jacobian
+ * points.  Result k equals sb_msm_registered on row k; the rows are sorted and reduced together (sub-batches sized from free
+ * device memory, sb_set_tuning(14) caps them).  count == 0 writes nothing. */
+int sb_msm_registered_batch(sb_ctx* ctx, uint64_t handle, uint64_t first, const uint8_t* scalars, uint32_t scalar_bytes,
+                            uint64_t n, uint32_t count, uint8_t* out);
 int sb_msm_sum_partials(sb_ctx* ctx, int group, const uint8_t* partials, int count, uint8_t* out);
 uint32_t sb_msm_partial_bytes(sb_ctx* ctx, int group);
 
@@ -111,6 +116,14 @@ int sb_groth16_prove_wtns(sb_ctx* ctx, uint64_t handle, const uint8_t* wtns, uin
 /* same proof with the witness uploaded by the previous sb_groth16_prove on this handle still resident in HBM
  * (no host->device copy): the device-resident timing bench.py reports as `value`. */
 int sb_groth16_prove_resident(sb_ctx* ctx, uint64_t handle, const uint8_t r[32], const uint8_t s[32], uint8_t* proof_affine_out);
+/* count proofs against one loaded (unsharded) Groth16 key.  witnesses = count * n_witness * 32 bytes (section-2 payloads,
+ * back to back); r, s = count * 32 bytes (Montgomery Fr); proofs_out = count * 8*n8q bytes, each laid out as sb_groth16_prove's.
+ * Proof k is byte-identical to sb_groth16_prove(witness k, r k, s k).  The proofs run in sub-batches sized from free device
+ * memory (sb_set_tuning(14) caps them); each sub-batch runs the QAP, NTT and MSM kernels once over all its proofs.  The
+ * resident witness of sb_groth16_prove_resident is left as it was.  count == 0 writes nothing; a wrong n_witness gives
+ * "Invalid witness length. Circuit: N, witness: M"; a sharded key is refused.  sb_last_ms(0) = the whole call. */
+int sb_groth16_prove_batch(sb_ctx* ctx, uint64_t handle, const uint8_t* witnesses, uint64_t n_witness, uint32_t count,
+                           const uint8_t* r, const uint8_t* s, uint8_t* proofs_out);
 int sb_groth16_release(sb_ctx* ctx, uint64_t handle);
 /* ---- PLONK (src/plonk_prove.js:47-889), next-tier path per SURVEY §8f rank 3 ----------------------------------
  * sb_plonk_load: a PLONK zkey (protocol id 2, sections 2-14: src/zkey_utils.js:261-299, src/plonk_constants.js) goes to
@@ -225,6 +238,8 @@ double sb_calibrate(sb_ctx* ctx, int what);
  *      is chosen: per chunk for MSMs on unregistered bases, and for window tables when they are built, i.e. when bases are
  *      registered or a key is loaded; a table keeps the c in force at that moment.  Tables are still skipped when
  *      W * n >= 2^31.  A large c costs memory: a plain MSM allocates W * 2^(c-1) buckets.
+ *  14  most proofs per sub-batch of sb_groth16_prove_batch, and rows per sub-batch of sb_msm_registered_batch (test hook;
+ *      0 = default: as many as the 32-bit bucket keys and free device memory allow)
  * The Python mirror applies SB_TUNE="key=value,..." from the environment when it loads the library. */
 int sb_set_tuning(int key, int value);
 /* synthetic bases for tests/benchmarks: chunks of 4096 points P_{c,j} = (k0(seed, c) + j*kd(seed)) * G, affine Montgomery, computed

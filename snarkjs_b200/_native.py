@@ -31,6 +31,7 @@ _SIGNATURES = {
     "sb_bases_release": (ctypes.c_int, [vp, u64]),
     "sb_msm_registered": (ctypes.c_int, [vp, u64, u64, vp, u32, u64, vp]),
     "sb_msm_registered_partial": (ctypes.c_int, [vp, u64, u64, vp, u32, u64, vp]),
+    "sb_msm_registered_batch": (ctypes.c_int, [vp, u64, u64, vp, u32, u64, u32, vp]),
     "sb_msm_sum_partials": (ctypes.c_int, [vp, ctypes.c_int, vp, ctypes.c_int, vp]),
     "sb_msm_partial_bytes": (u32, [vp, ctypes.c_int]),
     "sb_ntt_fr": (ctypes.c_int, [vp, vp, u64, ctypes.c_int, vp]),
@@ -47,6 +48,7 @@ _SIGNATURES = {
     "sb_groth16_info": (ctypes.c_int, [vp, u64, ctypes.POINTER(u32), ctypes.POINTER(u32), ctypes.POINTER(u32)]),
     "sb_groth16_prove": (ctypes.c_int, [vp, u64, vp, u64, vp, vp, vp]),
     "sb_groth16_prove_wtns": (ctypes.c_int, [vp, u64, vp, u64, vp, vp, vp]),
+    "sb_groth16_prove_batch": (ctypes.c_int, [vp, u64, vp, u64, u32, vp, vp, vp]),
     "sb_groth16_release": (ctypes.c_int, [vp, u64]),
     "sb_plonk_load": (ctypes.c_int, [vp, vp, u64, ctypes.POINTER(u64)]),
     "sb_plonk_load_file": (ctypes.c_int, [vp, ctypes.c_char_p, ctypes.POINTER(u64)]),

@@ -10,6 +10,10 @@
 #include <mutex>
 #include <future>
 #include <thread>
+#include <functional>
+#include <condition_variable>
+#include <deque>
+#include <memory>
 #include <dlfcn.h>
 #include <nccl.h>      // types and prototypes only: the library is dlopen'ed on first use (no link-time dependency)
 #include <fcntl.h>
@@ -75,6 +79,8 @@ struct Groth16Key {
     bool witness_resident = false;   // set by the first upload: sb_groth16_prove_resident refuses to run before it
     void *dW = nullptr, *dA_T = nullptr, *dB_T = nullptr, *dC_T = nullptr, *dTmp = nullptr, *dTmp2 = nullptr, *dTmp3 = nullptr, *dWsum = nullptr;
     size_t wsum_bytes = 0;           // size of dWsum (groth16_wsum_room grows it)
+    // sb_groth16_prove_batch, grown to the largest sub-batch: K' witnesses, the 3K' transforms and their scratch
+    DevBuf batchW, batchX, batchY;
 };
 
 }  // namespace
@@ -368,6 +374,7 @@ void prof_end(sb_ctx* c) {
 int g_serial_prove = 0;     // key 2: run every stream of a Groth16 prove call serialised on one stream (per-kernel-class timing)
 int g_no_tables = 0;        // key 3: ignore the precomputed window tables
 int g_msm_chunk_log = 0;    // key 6: log2 of the points per MSM chunk, 0 = 23 (a test hook)
+int g_batch_cap = 0;        // key 14: most proofs (MSM rows) per sub-batch of the batch entries, 0 = as many as memory takes
 
 // Precomputed window tables (msm.cuh k_precompute).  Built for sets of >= 2^12 points whose table index fits the
 // 31-bit entry value; g_no_tables disables them (plain windowed Pippenger on the raw bases).
@@ -459,6 +466,7 @@ int msm_host_inputs(sb_ctx* c, int group, const uint8_t* bases, const void* d_ba
 void free_key(Groth16Key* k) {
     for (void* p : {k->tA, k->tB1, k->tB2, k->tC, k->tH, k->dA, k->dB1, k->dB2, k->dC, k->dH, (void*)k->d_rowptr, (void*)k->d_sig, k->d_coef, k->dW, k->dA_T, k->dB_T, k->dC_T, k->dTmp, k->dTmp2, k->dTmp3, k->dWsum})
         if (p) cudaFree(p);
+    k->batchW.release(); k->batchX.release(); k->batchY.release();
     delete k;
 }
 
@@ -578,6 +586,123 @@ int sb_msm_registered(sb_ctx* c, uint64_t h, uint64_t first, const uint8_t* scal
 }
 int sb_msm_registered_partial(sb_ctx* c, uint64_t h, uint64_t first, const uint8_t* scalars, uint32_t sb, uint64_t n, uint8_t* partial) { SB_LOCK(c);
     return msm_registered_impl(c, h, first, scalars, sb, n, nullptr, partial);
+}
+// A fixed set of host threads draining one FIFO of tasks: the host work of a Groth16 batch (fixed parts, recombination,
+// assembly) never runs on more threads than the machine has cores, however many sub-batches are in flight.  The destructor
+// runs whatever is still queued before it joins, so tasks may reference locals declared before the pool.
+class HostPool {
+public:
+    explicit HostPool(unsigned n) { for (unsigned i = 0; i < std::max(1u, n); i++) th_.emplace_back([this]() { run(); }); }
+    ~HostPool() {
+        { std::lock_guard<std::mutex> l(mu_); stop_ = true; }
+        cv_.notify_all();
+        for (auto& t : th_) t.join();
+    }
+    void submit(std::function<void()> f) {
+        { std::lock_guard<std::mutex> l(mu_); q_.push_back(std::move(f)); pending_++; }
+        cv_.notify_one();
+    }
+    void wait() { std::unique_lock<std::mutex> l(mu_); idle_.wait(l, [this]() { return pending_ == 0; }); }
+private:
+    void run() {
+        for (;;) {
+            std::function<void()> f;
+            { std::unique_lock<std::mutex> l(mu_);
+              cv_.wait(l, [this]() { return stop_ || !q_.empty(); });
+              if (q_.empty()) return;
+              f = std::move(q_.front()); q_.pop_front(); }
+            f();
+            { std::lock_guard<std::mutex> l(mu_); if (--pending_ == 0) idle_.notify_all(); }
+        }
+    }
+    std::mutex mu_; std::condition_variable cv_, idle_;
+    std::deque<std::function<void()>> q_; size_t pending_ = 0; bool stop_ = false;
+    std::vector<std::thread> th_;
+};
+
+// Device bytes of one MSM over `entries` sorted (digit, point) entries into `buckets` buckets of `xb`-byte points: keys and
+// values double-buffered and about as much again for the radix sort's temporary storage (20 B per entry), the buckets, the
+// accumulation's head partials (<= one per 16 entries) with their keys, and the reduction's scratch (< 1/4 of the buckets).
+static size_t msm_batch_bytes(uint64_t entries, uint64_t buckets, size_t xb) {
+    return (size_t)(buckets + buckets / 4 + entries / 16 + 64) * xb + entries / 2;
+}
+static size_t sort_batch_bytes(uint64_t entries) { return (size_t)entries * 20; }
+
+// Proofs (or MSM rows) per sub-batch: what the 32-bit bucket keys allow, what fits in 85 % of the free device memory plus
+// what the context's grow-only buffers already hold (they are reallocated, not added), and the sb_set_tuning(14) cap.
+static uint32_t batch_size(sb_ctx* c, uint32_t count, uint64_t key_limit, size_t per_item, size_t held) {
+    uint64_t kb = std::min<uint64_t>(count, key_limit);
+    if (g_batch_cap > 0) kb = std::min<uint64_t>(kb, (uint64_t)g_batch_cap);
+    size_t free_b = 0, total_b = 0;
+    if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) { cudaGetLastError(); free_b = 0; }
+    held += c->sort_scratch.cap + c->sort_scratch2.cap + c->bucket_scratch.cap;
+    for (const MsmScratch& b : c->bscr) held += b.cap;
+    const size_t budget = (size_t)((double)(free_b + held) * 0.85);
+    kb = std::min<uint64_t>(kb, budget / std::max<size_t>(per_item, 1));
+    return (uint32_t)std::max<uint64_t>(kb, 1);
+}
+
+// count MSMs over the same registered bases: the rows are sorted and reduced together in sub-batches (MsmGeom::K), each row
+// recombined on its own.  Rows longer than an MSM chunk (2^23 points) go one by one through sb_msm_registered's path.
+int sb_msm_registered_batch(sb_ctx* c, uint64_t h, uint64_t first, const uint8_t* scalars, uint32_t sb, uint64_t n, uint32_t count, uint8_t* out) { SB_LOCK(c);
+    if (!c || h == 0 || h > c->bases.size() || !c->bases[h - 1].d) return fail(c, SB_ERR_ARG, "invalid bases handle");
+    const BaseSet& b = c->bases[h - 1];
+    if (first + n > b.n) return fail(c, SB_ERR_ARG, "registered base range out of bounds");
+    if (count == 0) return SB_OK;
+    if (!out || (n && !scalars)) return fail(c, SB_ERR_ARG, "null argument");
+    const GroupOps& G = b.group == SB_G1 ? c->g1 : c->g2;
+    const size_t jb = (size_t)3 * (G.aff_bytes / 2);   // normalised Jacobian output point
+    std::vector<uint8_t> acc(G.xyzz_bytes, 0);
+    if (n == 0) { for (uint32_t i = 0; i < count; i++) G.to_jacobian(acc.data(), out + i * jb); return SB_OK; }
+    if (sb == 0 || sb > 64) return fail(c, SB_ERR_ARG, "Scalar size does not match");
+    cudaSetDevice(c->device);
+    const uint64_t MAXC = 1ull << (g_msm_chunk_log > 0 ? g_msm_chunk_log : 23);
+    if (n > MAXC) {
+        tick(c, 4);
+        for (uint32_t i = 0; i < count; i++) { int rc = msm_registered_impl(c, h, first, scalars + (size_t)i * n * sb, sb, n, out + i * jb, nullptr); if (rc) return rc; }
+        tick(c, 5); cudaEventSynchronize(c->ev[5]); c->last_ms[0] = elapsed(c, 4, 5);
+        return SB_OK;
+    }
+    const bool table = b.table && sb <= 32;
+    MsmGeom g = msm_geometry(n, sb, c->fr_bits);
+    if (table) { g = b.gp; g.first = first; g.W = (int)((8 * sb + 1 + g.c - 1) / g.c); }
+    const void* d_bases = table ? b.table : (const void*)((const uint8_t*)b.d + first * G.aff_bytes);
+    const uint64_t e = n * (uint64_t)g.W;
+    const size_t per_row = (size_t)n * sb + sort_batch_bytes(e) + msm_batch_bytes(e, (uint64_t)g.windows_per_proof() * g.B, G.xyzz_bytes);
+    const uint32_t KB = batch_size(c, count, msm_batch_limit(n, g.c, g.W, g.precomp), per_row, c->io[1].cap + c->io[3].cap);
+    const size_t wrow = (size_t)msm_wsum_parts(g) * g.windows_per_proof() * G.xyzz_bytes;   // window-sum bytes of one row
+    tick(c, 0);
+    prof_begin(c);
+    for (uint32_t r0 = 0; r0 < count; r0 += KB) {
+        const uint32_t kb = std::min(KB, count - r0);
+        MsmGeom gK = g; gK.K = kb;
+        uint8_t* d_sc = (uint8_t*)c->io[1].get((size_t)kb * n * sb);
+        void* d_wsum = c->io[3].get(kb * wrow);
+        if (!d_sc || !d_wsum) return fail(c, SB_ERR_NOMEM, "out of device memory");
+        CU(c, h2d(c, d_sc, scalars + (size_t)r0 * n * sb, (size_t)kb * n * sb));
+        MsmSorted srt;
+        int rc = msm_sort_entries(d_sc, sb, n, gK, c->sort_scratch, c->stream, &srt, &c->stats);
+        if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
+        c->stats.cur_tag = (&G == &c->g1) ? SB_G1 : SB_G2;
+        rc = G.buckets(d_bases, srt, c->bucket_scratch, c->stream, d_wsum, &c->stats, nullptr, nullptr);
+        if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_buckets");
+        std::vector<uint8_t> ws(kb * wrow);
+        uint64_t entries = 0;
+        CU(c, cudaMemcpyAsync(ws.data(), d_wsum, ws.size(), cudaMemcpyDeviceToHost, c->stream));
+        CU(c, cudaMemcpyAsync(&entries, srt.counts, 8, cudaMemcpyDeviceToHost, c->stream));
+        CU(c, cudaStreamSynchronize(c->stream));
+        c->stat[(&G == &c->g1) ? 4 : 5] += (double)entries;
+        for (uint32_t q = 0; q < kb; q++) {
+            std::fill(acc.begin(), acc.end(), 0);
+            G.combine(ws.data() + q * wrow, g, acc.data());
+            G.to_jacobian(acc.data(), out + (size_t)(r0 + q) * jb);
+        }
+    }
+    tick(c, 1);
+    CU(c, cudaEventSynchronize(c->ev[1]));
+    prof_end(c);
+    c->last_ms[0] = elapsed(c, 0, 1);
+    return SB_OK;
 }
 uint32_t sb_msm_partial_bytes(sb_ctx* c, int group) { return c ? (group == SB_G1 ? c->g1.xyzz_bytes : c->g2.xyzz_bytes) : 0; }
 int sb_msm_sum_partials(sb_ctx* c, int group, const uint8_t* partials, int count, uint8_t* out) { SB_LOCK(c);
@@ -798,6 +923,7 @@ int sb_set_tuning(int key, int value) {
     case 7: if (value < 10 || value > 12) return SB_ERR_ARG; g_ntt_tile_log = value; return 0;         // NTT tile size
     case 8: g_stage_enabled = value; return 0;                                                          // pinned staging of pageable buffers
     case 13: if (value != 0 && (value < 3 || value > 22)) return SB_ERR_ARG; g_msm_force_c = value; return 0;   // MSM window bits
+    case 14: if (value < 0) return SB_ERR_ARG; g_batch_cap = value; return 0;                                    // proofs per sub-batch
     default: return SB_ERR_ARG;
     }
 }
@@ -1071,7 +1197,7 @@ static int groth16_device(sb_ctx* c, Groth16Key* k, const uint8_t* witness, uint
         if (m) {
             // buildABC1 (:147-187)
             { ProfScope pq(&c->stats, PROF_QAP, c->stream);
-              rc = fr_qap_rows(cv, k->d_rowptr, k->d_sig, k->d_coef, k->dW, k->dA_T, k->dB_T, k->dC_T, n, c->stream); c->launches++;
+              rc = fr_qap_rows(cv, k->d_rowptr, k->d_sig, k->d_coef, k->dW, nv, k->dA_T, k->dB_T, k->dC_T, n, 1, c->stream); c->launches++;
               pq.end(); }
             if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_qap_rows");
             // :64-76  ifft -> batchApplyKey(1, inc) -> fft, with 1/n of the inverse folded into the coset table
@@ -1297,7 +1423,9 @@ static int groth16_assemble_host(int curve, const GroupOps& G1, const GroupOps& 
 // The bracketed fixed parts depend only on the key and (r, s): a helper thread computes them while the GPU works;
 // the C bracket is folded by groth16_device (ProofScalars) as A and B1 land.  Same group elements, same proof bytes.
 struct FixedParts { std::vector<uint8_t> Fa, Fb, Fc; };
-static FixedParts groth16_fixed_parts(int curve, const GroupOps& G1, const GroupOps& G2, const VkPoints vk, const uint8_t* r, const uint8_t* s) {
+// g2_thread: the G2 multiple runs on a thread of its own (a single proof's latency); false runs it in place (batch pool)
+static FixedParts groth16_fixed_parts(int curve, const GroupOps& G1, const GroupOps& G2, const VkPoints vk, const uint8_t* r, const uint8_t* s,
+                                      bool g2_thread = true) {
     const uint32_t x1 = G1.xyzz_bytes, x2 = G2.xyzz_bytes;
     uint8_t rp[32], sp[32], rsp[32];
     plain_scalars(curve, r, s, rp, sp, rsp, false);
@@ -1305,7 +1433,7 @@ static FixedParts groth16_fixed_parts(int curve, const GroupOps& G1, const Group
     std::vector<uint8_t> a1(x1), b1(x1), d1(x1), b2(x2), d2(x2), t1(x1), t2(x2);
     G1.from_affine(vk.alpha1, a1.data()); G1.from_affine(vk.beta1, b1.data()); G1.from_affine(vk.delta1, d1.data());
     G2.from_affine(vk.beta2, b2.data()); G2.from_affine(vk.delta2, d2.data());
-    std::future<void> g2 = std::async(std::launch::async, [&]() { G2.times(d2.data(), sp, 32, t2.data()); });   // the one G2 multiple, on its own thread
+    std::future<void> g2 = std::async(g2_thread ? std::launch::async : std::launch::deferred, [&]() { G2.times(d2.data(), sp, 32, t2.data()); });   // the one G2 multiple
     G1.times(d1.data(), rp, 32, t1.data()); f.Fa = a1; G1.add(f.Fa.data(), t1.data());
     G1.times(a1.data(), sp, 32, f.Fc.data());
     G1.times(b1.data(), rp, 32, t1.data()); G1.add(f.Fc.data(), t1.data());
@@ -1333,6 +1461,192 @@ static int groth16_prove_folded(sb_ctx* c, Groth16Key* k, const uint8_t* witness
     if (rc) return rc;
     groth16_finish_folded(c->g1, c->g2, f, partials.data(), proof);
     return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------- Groth16 batches
+// sb_groth16_prove_batch: K proofs against one key, sub-batch by sub-batch.  A sub-batch of K' proofs runs the single-proof
+// pipeline once with K' times the work per launch: one QAP launch over K' witnesses, one strided NTT batch of 3K'
+// transforms per pass, one joinABC over K'n elements, one sort of the K' witnesses' digits (shared by A, B1, B2 and C) and
+// one of the K' H-scalar vectors, five bucket pipelines whose windows are the K' proofs' windows side by side
+// (MsmGeom::K), one download of the window sums.  Recombination and proof assembly run per proof on host threads.
+
+// What one more proof of a sub-batch costs in device memory: its witness, six n-element arrays (the 3n transform data and
+// its 3n scratch; the H scalars reuse the scratch), the sorted entries of its witness and H digits, and its share of the
+// five bucket pipelines (K'·B XYZZ buckets per MSM, G1 and G2).
+static size_t groth16_batch_footprint(const sb_ctx* c, const Groth16Key* k, const MsmGeom& gw, const MsmGeom& gh) {
+    const uint64_t n = k->domainSize, nv = k->nVars;
+    const size_t x1 = c->g1.xyzz_bytes, x2 = c->g2.xyzz_bytes;
+    const uint64_t ew = nv * (uint64_t)gw.W, eh = n * (uint64_t)gh.W;
+    const uint64_t bw = (uint64_t)gw.windows_per_proof() * gw.B, bh = (uint64_t)gh.windows_per_proof() * gh.B;
+    return (size_t)(nv + 6 * n) * 32 + sort_batch_bytes(ew) + sort_batch_bytes(eh)
+         + 3 * msm_batch_bytes(ew, bw, x1) + msm_batch_bytes(ew, bw, x2) + msm_batch_bytes(eh, bh, x1);
+}
+
+// Keys whose witness or H side is longer than one MSM chunk (2^23 points, sb_set_tuning(6) lowers it): the batched sort
+// would hold every entry of a proof at once, so each proof goes through the single-proof path, which cuts its MSMs into
+// chunks.  That path uploads to the key's resident witness buffer: the resident witness is saved first and put back after.
+static int groth16_prove_batch_chunked(sb_ctx* c, Groth16Key* k, const uint8_t* witnesses, uint32_t count,
+                                       const uint8_t* r, const uint8_t* s, uint8_t* proofs) {
+    const uint64_t nv = k->nVars;
+    const uint32_t proof_bytes = 2 * c->g1.aff_bytes + c->g2.aff_bytes;
+    const bool had = k->witness_resident;
+    void* saved = had ? k->batchW.get(nv * 32) : nullptr;
+    if (had && !saved) return fail(c, SB_ERR_NOMEM, "out of device memory (resident witness copy)");
+    tick(c, 5);
+    if (had) CU(c, cudaMemcpyAsync(saved, k->dW, nv * 32, cudaMemcpyDeviceToDevice, c->stream));
+    int rc = 0;
+    for (uint32_t i = 0; i < count && !rc; i++)
+        rc = groth16_prove_folded(c, k, witnesses + (size_t)i * nv * 32, nv, r + 32 * (size_t)i, s + 32 * (size_t)i, proofs + (size_t)i * proof_bytes);
+    if (had) { CU(c, cudaMemcpyAsync(k->dW, saved, nv * 32, cudaMemcpyDeviceToDevice, c->stream)); CU(c, cudaStreamSynchronize(c->stream)); }
+    k->witness_resident = had;
+    if (rc) return rc;
+    tick(c, 6);
+    CU(c, cudaEventSynchronize(c->ev[6]));
+    c->last_ms[0] = elapsed(c, 5, 6);
+    return 0;
+}
+
+static int groth16_prove_batch_impl(sb_ctx* c, Groth16Key* k, const uint8_t* witnesses, uint32_t count,
+                                    const uint8_t* r, const uint8_t* s, uint8_t* proofs) {
+    cudaSetDevice(c->device);
+    const uint64_t n = k->domainSize, nv = k->nVars;
+    const uint64_t MAXC = 1ull << (g_msm_chunk_log > 0 ? g_msm_chunk_log : 23);
+    if (nv > MAXC || n > MAXC) return groth16_prove_batch_chunked(c, k, witnesses, count, r, s, proofs);
+    const int cv = c->curve;
+    const GroupOps G1 = c->g1, G2 = c->g2;
+    const uint32_t x1 = G1.xyzz_bytes, x2 = G2.xyzz_bytes, pb = 4 * x1 + x2, proof_bytes = 2 * G1.aff_bytes + G2.aff_bytes;
+    MsmGeom gw = msm_geometry(nv, 32, c->fr_bits), gh = msm_geometry(n, 32, c->fr_bits);
+    const bool pre = k->tA != nullptr;
+    if (pre) { gw = k->gpW; gw.first = 0; gh = k->gpH; gh.first = 0; }
+    // 3K' transforms per NTT launch: the grid's y dimension (65535) bounds K' as well
+    const uint64_t key_limit = std::min({msm_batch_limit(nv, gw.c, gw.W, gw.precomp), msm_batch_limit(n, gh.c, gh.W, gh.precomp), (uint64_t)65535 / 3});
+    const uint32_t KB = batch_size(c, count, key_limit, groth16_batch_footprint(c, k, gw, gh), k->batchW.cap + k->batchX.cap + k->batchY.cap);
+    // per proof: the five partials A | B1 | C | H | B2, then the proof
+    std::vector<uint8_t> allp((size_t)count * pb, 0);
+    std::vector<FixedParts> fixed(count);
+    const VkPoints vk{k->alpha1.data(), k->beta1.data(), k->beta2.data(), k->delta1.data(), k->delta2.data()};
+    // Host work on one pool of at most one thread per core, declared after everything its tasks touch: leaving this
+    // function (also on an error) runs the queued tasks and joins.  The fixed parts go first, so they overlap the GPU work.
+    HostPool pool(std::min<unsigned>(count, std::max(1u, std::thread::hardware_concurrency())));
+    for (uint32_t i = 0; i < count; i++)
+        pool.submit([&, i]() { fixed[i] = groth16_fixed_parts(cv, G1, G2, vk, r + 32 * (size_t)i, s + 32 * (size_t)i, false); });
+    int rc;
+    tick(c, 0);
+    prof_begin(c);
+    cudaStream_t s0 = c->stream, sN = c->aux[5];
+    for (uint32_t k0 = 0; k0 < count; k0 += KB) {
+        const uint32_t kb = std::min(KB, count - k0);
+        MsmGeom gwK = gw, ghK = gh; gwK.K = kb; ghK.K = kb;
+        const size_t tn = (size_t)kb * n * 32;   // bytes of one of A, B, C over the sub-batch
+        uint8_t* dW = (uint8_t*)k->batchW.get((size_t)kb * nv * 32);
+        uint8_t* X = (uint8_t*)k->batchX.get(3 * tn);
+        uint8_t* Y = (uint8_t*)k->batchY.get(3 * tn);
+        if (!dW || !X || !Y) return fail(c, SB_ERR_NOMEM, "out of device memory (Groth16 batch of " + std::to_string(kb) + " proofs)");
+        CU(c, h2d(c, dW, witnesses + (size_t)k0 * nv * 32, (size_t)kb * nv * 32));
+        CU(c, cudaEventRecord(c->pev[0], s0));
+        CU(c, cudaStreamWaitEvent(sN, c->pev[0], 0));
+        // side stream: QAP rows -> iNTT -> coset NTT (1/n folded in) -> joinABC -> sort of the H scalars
+        { ProfScope pq(&c->stats, PROF_QAP, sN);
+          rc = fr_qap_rows(cv, k->d_rowptr, k->d_sig, k->d_coef, dW, nv, X, X + tn, X + 2 * tn, n, kb, sN); c->launches++;
+          pq.end(); }
+        if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_qap_rows");
+        const uint8_t* inc = (k->power == c->fr_s) ? c->shift.data() : c->roots[k->power + 1].data();
+        uint8_t ninv[32];
+        if (cv == SB_BN254) ninv_bytes<BnFr>(k->power, ninv); else ninv_bytes<BlsFr>(k->power, ninv);
+        FrPre fpre; rc = get_pre(c, n, ninv, inc, &fpre); if (rc) return rc;
+        FrNttTables tbi, tbf;
+        rc = get_ntt_tab(c, k->power, true, &tbi); if (rc) return rc;
+        rc = get_ntt_tab(c, k->power, false, &tbf); if (rc) return rc;
+        int side = 0, side2 = 0, launches = 0;
+        ProfScope pn(&c->stats, PROF_NTT, sN);
+        rc = fr_ntt_strided(cv, X, Y, 3 * (int)kb, k->power, &tbi, nullptr, nullptr, sN, &side, &launches);
+        if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_ntt_strided");
+        uint8_t* src = side ? Y : X; uint8_t* dst = side ? X : Y;
+        rc = fr_ntt_strided(cv, src, dst, 3 * (int)kb, k->power, &tbf, &fpre, nullptr, sN, &side2, &launches);
+        if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_ntt_strided");
+        pn.end();
+        c->launches += launches;
+        uint8_t* ev = side2 ? dst : src; uint8_t* hsc = side2 ? src : dst;   // coset evaluations; the H scalars go to the other half
+        { ProfScope pj(&c->stats, PROF_JOIN, sN);
+          rc = fr_join_abc(cv, ev, ev + tn, ev + 2 * tn, hsc, (uint64_t)kb * n, sN); c->launches++;
+          pj.end(); }
+        if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_join_abc");
+        MsmSorted sh;
+        rc = msm_sort_entries(hsc, 32, n, ghK, c->sort_scratch2, sN, &sh, &c->stats);
+        if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
+        CU(c, cudaEventRecord(c->pev[1], sN));
+        // main stream: the witness digits, sorted once for A, B1, B2 and C
+        MsmSorted sw;
+        rc = msm_sort_entries(dW, 32, nv, gwK, c->sort_scratch, s0, &sw, &c->stats);
+        if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
+        const size_t w1 = (size_t)gwK.wsum_points() * x1, w2 = (size_t)gwK.wsum_points() * x2, wh = (size_t)ghK.wsum_points() * x1;
+        const size_t wtot = 3 * w1 + w2 + wh;
+        rc = groth16_wsum_room(c, k, wtot, wtot + 64);
+        if (rc) return rc;
+        uint8_t* dws = (uint8_t*)k->dWsum; uint8_t* hws = c->pinned;
+        uint64_t* hcounts = (uint64_t*)(c->pinned + wtot);
+        struct Job { const GroupOps* G; const void* bases; size_t off; size_t len; int tag; const MsmSorted* srt; };
+        const Job jobs[5] = {{&G1, pre ? k->tA : k->dA, 0, w1, SB_G1, &sw},
+                             {&G1, pre ? k->tB1 : k->dB1, w1, w1, SB_G1, &sw},
+                             {&G2, pre ? k->tB2 : k->dB2, 3 * w1, w2, SB_G2, &sw},
+                             {&G1, pre ? k->tC : k->dC, 2 * w1, w1, SB_G1, &sw},
+                             {&G1, pre ? k->tH : k->dH, 3 * w1 + w2, wh, SB_G1, &sh}};
+        for (int i = 0; i < 5; i++) {
+            cudaStream_t st = c->aux[i];
+            if (i == 4) CU(c, cudaStreamWaitEvent(s0, c->pev[1], 0));   // H needs the NTT chain
+            c->stats.cur_tag = jobs[i].tag;
+            rc = jobs[i].G->buckets(jobs[i].bases, *jobs[i].srt, c->bscr[i], s0, dws + jobs[i].off, &c->stats, st, c->pev[8 + i]);
+            if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_buckets");
+            CU(c, cudaMemcpyAsync(hws + jobs[i].off, dws + jobs[i].off, jobs[i].len, cudaMemcpyDeviceToHost, st));
+            if (i == 0) CU(c, cudaMemcpyAsync(&hcounts[0], sw.counts, 8, cudaMemcpyDeviceToHost, st));
+            if (i == 4) CU(c, cudaMemcpyAsync(&hcounts[1], sh.counts, 8, cudaMemcpyDeviceToHost, st));
+            CU(c, cudaEventRecord(c->pev[2 + i], st));
+        }
+        for (int i = 0; i < 5; i++) { CU(c, cudaEventSynchronize(c->pev[2 + i])); CU(c, cudaStreamWaitEvent(s0, c->pev[2 + i], 0)); }
+        c->stat[4] += 3.0 * (double)hcounts[0] + (double)hcounts[1]; c->stat[5] += (double)hcounts[0];
+        // the pinned area serves the next sub-batch: the host work gets its own copy and runs while the GPU goes on.
+        // Proof q's window sums start q * windows_per_proof * msm_wsum_parts points into each MSM's region.
+        auto host = std::make_shared<std::vector<uint8_t>>(hws, hws + wtot);
+        const size_t sw1 = (size_t)msm_wsum_parts(gw) * gw.windows_per_proof(), swh = (size_t)msm_wsum_parts(gh) * gh.windows_per_proof();
+        size_t offs[5];
+        const size_t per[5] = {sw1 * x1, sw1 * x1, sw1 * x2, sw1 * x1, swh * x1};
+        for (int i = 0; i < 5; i++) offs[i] = jobs[i].off;
+        for (uint32_t p = k0; p < k0 + kb; p++) pool.submit([&, host, p, k0, offs, per]() {
+            const size_t q = p - k0;
+            const uint8_t* ws = host->data();
+            uint8_t* pA = allp.data() + (size_t)p * pb; uint8_t* pB1 = pA + x1; uint8_t* pC = pB1 + x1; uint8_t* pH = pC + x1; uint8_t* pB2 = pH + x1;
+            G1.combine(ws + offs[0] + q * per[0], gw, pA);
+            G1.combine(ws + offs[1] + q * per[1], gw, pB1);
+            G2.combine(ws + offs[2] + q * per[2], gw, pB2);
+            G1.combine(ws + offs[3] + q * per[3], gw, pC);
+            G1.combine(ws + offs[4] + q * per[4], gh, pH);
+            // C' = C + H + s*A + r*B1, as groth16_device folds it
+            ProofScalars ps; uint8_t rsp[32]; plain_scalars(cv, r + 32 * (size_t)p, s + 32 * (size_t)p, ps.rp, ps.sp, rsp, false);
+            std::vector<uint8_t> t(x1);
+            G1.add(pC, pH);
+            G1.times(pA, ps.sp, 32, t.data()); G1.add(pC, t.data());
+            G1.times(pB1, ps.rp, 32, t.data()); G1.add(pC, t.data());
+        });
+    }
+    pool.wait();   // every fixed part and every folded partial
+    for (uint32_t p = 0; p < count; p++)
+        pool.submit([&, p]() { groth16_finish_folded(G1, G2, fixed[p], allp.data() + (size_t)p * pb, proofs + (size_t)p * proof_bytes); });
+    pool.wait();
+    tick(c, 1);
+    CU(c, cudaEventSynchronize(c->ev[1]));
+    prof_end(c);
+    c->last_ms[0] = elapsed(c, 0, 1);
+    return 0;
+}
+
+int sb_groth16_prove_batch(sb_ctx* c, uint64_t h, const uint8_t* witnesses, uint64_t n_witness, uint32_t count,
+                           const uint8_t* r, const uint8_t* s, uint8_t* proofs) { SB_LOCK(c);
+    Groth16Key* k = get_key(c, h); if (!k) return fail(c, SB_ERR_ARG, "invalid groth16 handle");
+    if (k->n_shards > 1) return fail(c, SB_ERR_ARG, "proving key was loaded sharded: use sb_groth16_prove_shard + sb_groth16_finish");
+    if (n_witness != k->nVars) return fail(c, SB_ERR_ARG, "Invalid witness length. Circuit: " + std::to_string(k->nVars) + ", witness: " + std::to_string(n_witness));
+    if (count == 0) return SB_OK;
+    if (!witnesses || !r || !s || !proofs) return fail(c, SB_ERR_ARG, "null argument");
+    return groth16_prove_batch_impl(c, k, witnesses, count, r, s, proofs);
 }
 
 int sb_groth16_prove(sb_ctx* c, uint64_t h, const uint8_t* witness, uint64_t n_witness, const uint8_t r[32], const uint8_t s[32], uint8_t* proof) { SB_LOCK(c);

@@ -15,11 +15,15 @@ int fr_ntt(int curve, void* a, void* b, int L, const FrNttTables* tb, const FrPr
 // batched variant: count (<= 4) transforms of size 2^L; a[i] input, b[i] scratch; *side = 0 results in a[], 1 in b[]
 int fr_ntt_batch(int curve, void* const* a, void* const* b, int count, int L, const FrNttTables* tb, const FrPre* pre, const void* post_scale,
                  cudaStream_t stream, int* side, int* launches);
+// count (<= 65535) contiguous transforms of size 2^L: a = count * 2^L inputs back to back, b = as much scratch; *side as above
+int fr_ntt_strided(int curve, void* a, void* b, int count, int L, const FrNttTables* tb, const FrPre* pre, const void* post_scale,
+                   cudaStream_t stream, int* side, int* launches);
 // number of passes fr_ntt / fr_ntt_batch run for size 2^L (the result lands in the scratch buffers iff it is odd)
 int fr_ntt_passes(int L);
 int fr_apply_key(int curve, const void* in, void* out, uint64_t n, const FrPre* t, cudaStream_t stream);
 int fr_convert(int curve, const void* in, void* out, uint64_t n, int to_mont, cudaStream_t stream);
 int fr_join_abc(int curve, const void* a, const void* b, const void* c, void* out, uint64_t n, cudaStream_t stream);
-int fr_qap_rows(int curve, const uint64_t* row_ptr, const uint32_t* sig, const void* coef, const void* witness,
-                void* A, void* B, void* C, uint64_t n, cudaStream_t stream);
+// K proofs: witness k (n_witness elements) at witness + k * n_witness; its A/B/C rows at A/B/C + k * n
+int fr_qap_rows(int curve, const uint64_t* row_ptr, const uint32_t* sig, const void* coef, const void* witness, uint64_t n_witness,
+                void* A, void* B, void* C, uint64_t n, uint32_t K, cudaStream_t stream);
 }

@@ -30,6 +30,17 @@ int fr_ntt_batch(int curve, void* const* a, void* const* b, int count, int L, co
         return (int)cudaGetLastError();
     })
 }
+int fr_ntt_strided(int curve, void* a, void* b, int count, int L, const FrNttTables* tb, const FrPre* pre, const void* post_scale,
+                   cudaStream_t stream, int* side, int* launches) {
+    if (count < 1 || count > 65535 || L < 0) return -1;
+    FR_DISPATCH(curve, {
+        NttTables<F> t; t.tw_lo = (const F*)tb->tw_lo; t.tw_hi = (const F*)tb->tw_hi; t.h = tb->h; t.wr = (const F*)tb->wr;
+        NttPre<F> p; if (pre) { p.lo = (const F*)pre->lo; p.hi = (const F*)pre->hi; p.h = pre->h; }
+        F* aa[1] = {(F*)a}; F* bb[1] = {(F*)b};
+        *side = ntt_run_batch<F>(aa, bb, count, L, t, pre ? &p : nullptr, (const F*)post_scale, stream, launches, 1ull << L);
+        return (int)cudaGetLastError();
+    })
+}
 int fr_ntt_passes(int L) { return ntt_plan(L).npass; }
 int fr_apply_key(int curve, const void* in, void* out, uint64_t n, const FrPre* t, cudaStream_t stream) {
     FR_DISPATCH(curve, {
@@ -50,10 +61,12 @@ int fr_join_abc(int curve, const void* a, const void* b, const void* c, void* ou
         return (int)cudaGetLastError();
     })
 }
-int fr_qap_rows(int curve, const uint64_t* row_ptr, const uint32_t* sig, const void* coef, const void* witness,
-                void* A, void* B, void* C, uint64_t n, cudaStream_t stream) {
+int fr_qap_rows(int curve, const uint64_t* row_ptr, const uint32_t* sig, const void* coef, const void* witness, uint64_t n_witness,
+                void* A, void* B, void* C, uint64_t n, uint32_t K, cudaStream_t stream) {
     FR_DISPATCH(curve, {
-        if (n) k_qap_rows<F><<<(unsigned)((n + 127) / 128), 128, 0, stream>>>(row_ptr, sig, (const F*)coef, (const F*)witness, (F*)A, (F*)B, (F*)C, n);
+        const unsigned grid = (unsigned)((n * K + 127) / 128);
+        if (n && K == 1) k_qap_rows<F, false><<<grid, 128, 0, stream>>>(row_ptr, sig, (const F*)coef, (const F*)witness, n_witness, (F*)A, (F*)B, (F*)C, n, 1);
+        else if (n && K) k_qap_rows<F, true><<<grid, 128, 0, stream>>>(row_ptr, sig, (const F*)coef, (const F*)witness, n_witness, (F*)A, (F*)B, (F*)C, n, K);
         return (int)cudaGetLastError();
     })
 }

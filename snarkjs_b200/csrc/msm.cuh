@@ -390,6 +390,9 @@ k_axis_tree(AxisJob j0, AxisJob j1) {
     if (lane == 0) store_vec((XYZZ<F>*)j.out + wid, acc);
 }
 
+// sb_set_tuning(1, 1): reduce the buckets with k_reduce / k_window_sum even where ws_plan accepts the geometry
+extern int g_msm_force_reduce;
+
 // Host plan of the axis-sum levels for one geometry.  Buckets of a window form H = 2^er rows... of 2^m columns
 // (m = WS_COL_BITS when the window has more than 2^m buckets, else there is no split and C = the buckets themselves).
 static constexpr int WS_COL_BITS = 10;
@@ -419,6 +422,10 @@ __host__ inline WsPlan ws_plan(const MsmGeom& g) {
     p.tw = 2 * NW * (p.nR + p.nC);
     return p;
 }
+// Points per window that msm_buckets writes as window sums, the layout msm_group.inl's combine reads: the five weighted
+// parts of k_ws_final, or one point (k_reduce / k_window_sum) when ws_plan rejects the geometry or sb_set_tuning(1, 1)
+// forces the running-sum reduction.  A batch's proof k starts at point k * windows_per_proof() * msm_wsum_parts(g).
+__host__ inline uint32_t msm_wsum_parts(const MsmGeom& g) { return (ws_plan(g).ok && !g_msm_force_reduce) ? 5u : 1u; }
 // scratch (in XYZZ elements) of the reduction: k_reduce partials, or the axis-sum ping-pong buffers + chunk pairs
 __host__ inline size_t msm_reduce_scratch_elems(const MsmGeom& g) {
     const uint32_t NW = g.windows();
@@ -497,8 +504,6 @@ struct MsmScratch {
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
 
-// sb_set_tuning(1, 1): reduce the buckets with k_reduce / k_window_sum even where ws_plan accepts the geometry
-extern int g_msm_force_reduce;
 
 struct MsmLaunchStats {
     int launches = 0;
@@ -614,7 +619,7 @@ int msm_buckets(const Affine<F>* d_bases, const MsmSorted& s, MsmScratch& scratc
     if (!heads0 && tail_stream && tail_stream != stream && ev_acc) { cudaEventRecord(ev_acc, stream); cudaStreamWaitEvent(tail_stream, ev_acc, 0); stream = tail_stream; }
     ProfScope pred(stats, g2 ? PROF_REDUCE_G2 : PROF_REDUCE, stream);
     const WsPlan wp = ws_plan(g);
-    if (wp.ok && !g_msm_force_reduce) {
+    if (msm_wsum_parts(g) == 5) {
         // axis sums (rows and columns of one level per launch), then the warp-shuffle weighted sums
         XYZZ<F>* rowb[2] = {partials, partials + wp.rowA};
         XYZZ<F>* colb[2] = {partials + wp.rowA + wp.rowB, partials + wp.rowA + wp.rowB + wp.colA};

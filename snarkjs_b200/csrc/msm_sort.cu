@@ -10,12 +10,19 @@ int g_msm_force_c = 0;
 // ------------------------------------------------------------------------------------------------
 // digits: thread i recodes scalar i into W signed digits (reference _getChunk extracts unsigned chunks;
 // signed recoding halves the bucket count and is free because negating an affine point is free).
-// entries are written window-major (keys[w*n + i]) so every store is coalesced.
+// entries are written window-major (keys[w*K*n + i]) so every store is coalesced.
+// A batch (g.K > 1) holds K vectors of n scalars back to back: scalar i = k*n + j of vector k lands in vector k's own bucket
+// sets (key offset k * windows_per_proof * B), and its value is point j (or table index of j): every vector shares the bases.
 // ------------------------------------------------------------------------------------------------
+// BATCH = false is a single vector (g.K = 1): no vector index to divide out.
+template <bool BATCH>
 __global__ void k_digits(const uint8_t* __restrict__ scalars, uint32_t sbytes, uint64_t n, MsmGeom g,
                          uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+    const uint64_t nk = n * g.K;
     uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-    if (i >= n) return;
+    if (i >= nk) return;
+    const uint64_t kp = BATCH ? i / n : 0, j = i - kp * n;
+    const uint32_t kbase = (uint32_t)kp * (g.precomp ? 1u : (uint32_t)g.W) * g.B;
     uint32_t w32[17];                       // up to 64-byte scalars + 1 guard word
     const uint8_t* s = scalars + i * sbytes;
     if (sbytes == 32 && ((uintptr_t)scalars & 15) == 0) {
@@ -35,12 +42,12 @@ __global__ void k_digits(const uint8_t* __restrict__ scalars, uint32_t sbytes, u
         uint32_t bit = (uint32_t)w * g.c, wi = bit >> 5, sh = bit & 31;
         uint64_t two = (uint64_t)w32[wi] | ((uint64_t)(wi + 1 < 17 ? w32[wi + 1] : 0) << 32);
         uint32_t raw = ((uint32_t)(two >> sh) & cmask) + carry;
-        uint32_t key, val = (uint32_t)i;
+        uint32_t key, val = (uint32_t)j;
         if (raw > half) { raw = (1u << g.c) - raw; carry = 1; val |= 0x80000000u; } else carry = 0;
-        if (g.precomp) { key = raw ? raw - 1 : MSM_INVALID_KEY; val = (uint32_t)((uint64_t)w * g.stride + g.first + i) | (val & 0x80000000u); }
-        else key = raw ? (uint32_t)w * g.B + raw - 1 : MSM_INVALID_KEY;
-        keys[(uint64_t)w * n + i] = key;
-        vals[(uint64_t)w * n + i] = val;
+        if (g.precomp) { key = raw ? kbase + raw - 1 : MSM_INVALID_KEY; val = (uint32_t)((uint64_t)w * g.stride + g.first + j) | (val & 0x80000000u); }
+        else key = raw ? kbase + (uint32_t)w * g.B + raw - 1 : MSM_INVALID_KEY;
+        keys[(uint64_t)w * nk + i] = key;
+        vals[(uint64_t)w * nk + i] = val;
     }
 }
 
@@ -68,9 +75,10 @@ __global__ void k_count_valid(const uint32_t* __restrict__ keys, uint64_t total,
 
 int msm_sort_entries(const uint8_t* d_scalars, uint32_t sbytes, uint64_t n, MsmGeom g, MsmScratch& scratch,
                      cudaStream_t stream, MsmSorted* out, MsmLaunchStats* stats) {
-    const uint64_t total = n * (uint64_t)g.W;
+    const uint64_t total = n * (uint64_t)g.K * (uint64_t)g.W;
     const uint64_t nbuckets = (uint64_t)g.windows() * g.B;
     if (sbytes == 0 || sbytes > 64) return (int)cudaErrorInvalidValue;
+    if (g.K < 1 || (g.K > 1 && g.K > msm_batch_limit(n, g.c, g.W, g.precomp))) return (int)cudaErrorInvalidValue;   // keys stay below INVALID
     int key_bits = 1; while ((1ull << key_bits) < nbuckets) key_bits++;
     int end_bit = key_bits + 1 > 32 ? 32 : key_bits + 1;   // INVALID (all ones) sorts after every valid key
     size_t sort_tmp = 0;
@@ -86,7 +94,9 @@ int msm_sort_entries(const uint8_t* d_scalars, uint32_t sbytes, uint64_t n, MsmG
     uint64_t* counts = (uint64_t*)(base + o_counts);
     int launches = 0;
     ProfScope prof(stats, PROF_SORT, stream);
-    k_digits<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(d_scalars, sbytes, n, g, keys0, vals0); launches++;
+    if (g.K > 1) k_digits<true><<<(unsigned)((n * g.K + 255) / 256), 256, 0, stream>>>(d_scalars, sbytes, n, g, keys0, vals0);
+    else k_digits<false><<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(d_scalars, sbytes, n, g, keys0, vals0);
+    launches++;
     kb = cub::DoubleBuffer<uint32_t>(keys0, keys1); vb = cub::DoubleBuffer<uint32_t>(vals0, vals1);
     cudaError_t e = cub::DeviceRadixSort::SortPairs(base + o_tmp, sort_tmp, kb, vb, (uint64_t)total, 0, end_bit, stream);
     if (e != cudaSuccess) return (int)e;

@@ -89,16 +89,19 @@ static constexpr uint32_t NTT_WR_BYTES = (1u << (NTT_DMAX - 1)) * 32;   // the i
 static constexpr size_t NTT_SMEM_EXTRA = NTT_WR_BYTES + 16;             // + the mbarrier
 
 // One Stockham pass.  Fr has 8 limbs for both supported curves.
-// up to 4 independent transforms of the same size per launch (blockIdx.y): Groth16 runs A, B and C together so that the
-// grid fills whole waves (512 CTAs of one 2^20 pass are 1.15 waves at 3 CTAs/SM; 1536 are 3.46)
-template <class F> struct NttBatch { const F* in[4]; F* out[4]; };
+// several independent transforms of the same size per launch (blockIdx.y): Groth16 runs A, B and C together so that the
+// grid fills whole waves (512 CTAs of one 2^20 pass are 1.15 waves at 3 CTAs/SM; 1536 are 3.46).  Up to 4 transforms
+// anywhere in memory (stride = 0: in[y], out[y]), or any number of contiguous ones (stride = 2^L: in[0] + y * stride), the
+// 3K transforms of a batch of K proofs.
+template <class F> struct NttBatch { const F* in[4]; F* out[4]; uint64_t stride; };
 
-template <class F>
+// STRIDED selects the addressing at compile time, so the single-proof launches (stride 0) run the code they always ran.
+template <class F, bool STRIDED>
 __global__ void __launch_bounds__(NTT_THREADS)
 k_ntt_pass(NttBatch<F> io, int L, int lgp, int deg, int logc,
            NttTables<F> tb, NttPre<F> pre, const F* __restrict__ post_scale) {
-    const F* __restrict__ in = io.in[blockIdx.y];
-    F* __restrict__ out = io.out[blockIdx.y];
+    const F* __restrict__ in = STRIDED ? io.in[0] + blockIdx.y * io.stride : io.in[blockIdx.y];
+    F* __restrict__ out = STRIDED ? io.out[0] + blockIdx.y * io.stride : io.out[blockIdx.y];
     extern __shared__ uint4 ntt_smem[];
     const uint32_t r = 1u << deg, C = 1u << logc, tile = r << logc;
     uint4* slo = ntt_smem; uint4* shi = ntt_smem + tile;
@@ -190,18 +193,22 @@ __global__ void k_join_abc(const F* __restrict__ a, const F* __restrict__ b, con
 }
 // buildABC1 (src/groth16_prove.js:147-187) as a CSR sparse mat-vec: rows 0..n-1 -> A, n..2n-1 -> B;
 // entry = (signal, coef*R^2); value = sum coef*R^2 (x) w[signal]  (Montgomery product with the plain
-// witness gives a Montgomery result); C = A (x) B.
-template <class F>
+// witness gives a Montgomery result); C = A (x) B.  K proofs: witness k at witness + k*nw, its rows at A/B/C + k*n.
+// BATCH = false is the single proof (K = 1): no proof index to divide out.
+template <class F, bool BATCH>
 __global__ void k_qap_rows(const uint64_t* __restrict__ row_ptr, const uint32_t* __restrict__ sig, const F* __restrict__ coef,
-                           const F* __restrict__ witness, F* __restrict__ A, F* __restrict__ B, F* __restrict__ Cc, uint64_t n) {
+                           const F* __restrict__ witness, uint64_t nw, F* __restrict__ A, F* __restrict__ B, F* __restrict__ Cc,
+                           uint64_t n, uint32_t K) {
     uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-    if (i >= n) return;
+    if (i >= n * K) return;
+    const uint64_t kp = BATCH ? i / n : 0, row = i - kp * n;
+    const F* __restrict__ wk = witness + kp * nw;
     F acc[2];
 #pragma unroll 1
     for (int m = 0; m < 2; m++) {
         F s = F::zero();
-        uint64_t lo = row_ptr[m * n + i], hi = row_ptr[m * n + i + 1];
-        for (uint64_t e = lo; e < hi; e++) s = F::add(s, F::mul(ldg_fe<F>(coef + e), ldg_fe<F>(witness + sig[e])));
+        uint64_t lo = row_ptr[m * n + row], hi = row_ptr[m * n + row + 1];
+        for (uint64_t e = lo; e < hi; e++) s = F::add(s, F::mul(ldg_fe<F>(coef + e), ldg_fe<F>(wk + sig[e])));
         acc[m] = s;
     }
     stg_fe<F>(A + i, acc[0]); stg_fe<F>(B + i, acc[1]);
@@ -229,11 +236,12 @@ inline NttPlan ntt_plan(int L) {
     return pl;
 }
 
-// Runs all passes over `count` (<= 4) transforms; a[i] holds input i, b[i] is its scratch; returns 0 if the results end
-// in a[], 1 if in b[].  pre/post optional.
+// Runs all passes over `count` transforms; a[i] holds input i, b[i] is its scratch; returns 0 if the results end
+// in a[], 1 if in b[].  pre/post optional.  stride = 0: count <= 4 separate arrays; stride = 2^L: a[0] and b[0] hold
+// `count` contiguous transforms each (count <= 65535, the grid's y limit).
 template <class F>
 int ntt_run_batch(F* const* a, F* const* b, int count, int L, const NttTables<F>& tb, const NttPre<F>* pre, const F* post_scale,
-                  cudaStream_t stream, int* launches) {
+                  cudaStream_t stream, int* launches, uint64_t stride = 0) {
     NttPlan pl = ntt_plan(L);
     int lgp = 0, side = 0;
     for (int i = 0; i < pl.npass; i++) {
@@ -243,9 +251,11 @@ int ntt_run_batch(F* const* a, F* const* b, int count, int L, const NttTables<F>
         dim3 grid((unsigned)((1ull << L) >> (deg + logc)), (unsigned)count);
         unsigned threads = tile / 2 < (unsigned)NTT_THREADS ? (tile / 2 < 32 ? 32 : tile / 2) : NTT_THREADS;
         NttBatch<F> io;
-        for (int k = 0; k < 4; k++) { int kk = k < count ? k : 0; io.in[k] = side ? b[kk] : a[kk]; io.out[k] = side ? a[kk] : b[kk]; }
+        for (int k = 0; k < 4; k++) { int kk = (k < count && !stride) ? k : 0; io.in[k] = side ? b[kk] : a[kk]; io.out[k] = side ? a[kk] : b[kk]; }
+        io.stride = stride;
         NttPre<F> p0; if (i == 0 && pre) p0 = *pre;
-        k_ntt_pass<F><<<grid, threads, smem, stream>>>(io, L, lgp, deg, logc, tb, p0, (i == pl.npass - 1) ? post_scale : nullptr);
+        if (stride) k_ntt_pass<F, true><<<grid, threads, smem, stream>>>(io, L, lgp, deg, logc, tb, p0, (i == pl.npass - 1) ? post_scale : nullptr);
+        else k_ntt_pass<F, false><<<grid, threads, smem, stream>>>(io, L, lgp, deg, logc, tb, p0, (i == pl.npass - 1) ? post_scale : nullptr);
         if (launches) (*launches)++;
         lgp += deg; side ^= 1;
     }
@@ -259,7 +269,9 @@ F* ntt_run(F* a, F* b, int L, const NttTables<F>& tb, const NttPre<F>* pre, cons
     return ntt_run_batch<F>(aa, bb, 1, L, tb, pre, post_scale, stream, launches) ? b : a;
 }
 template <class F> inline cudaError_t ntt_configure() {
-    return cudaFuncSetAttribute(k_ntt_pass<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(128 * 1024 + NTT_SMEM_EXTRA));
+    cudaError_t e = cudaFuncSetAttribute(k_ntt_pass<F, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(128 * 1024 + NTT_SMEM_EXTRA));
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(k_ntt_pass<F, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(128 * 1024 + NTT_SMEM_EXTRA));
 }
 
 }  // namespace sb

@@ -200,6 +200,24 @@ class Group:
         self._c.check(self._c.lib.sb_msm_registered(self._c.h, handle, first, _ptr(s), s.size // n, n, _ptr(out)))
         return out
 
+    def multiExpRegisteredBatch(self, handle: int, buffScalars, count: int, first: int = 0, n: int | None = None):
+        """count MSMs over the registered bases [first, first+n): buffScalars holds count rows of n scalars back to back.
+        Returns a (count, sJacobian) array; row k equals multiExpRegistered on scalar row k."""
+        s = _arr(buffScalars)
+        out = np.empty((count, self.sJacobian), np.uint8)
+        if count == 0:
+            return out
+        if n is None:
+            n = s.size // (32 * count)
+        if n == 0:
+            out[:] = np.frombuffer(self.zero, np.uint8)
+            return out
+        sb = s.size // (n * count)
+        if sb * n * count != s.size:
+            raise SbError("Scalar size does not match")
+        self._c.check(self._c.lib.sb_msm_registered_batch(self._c.h, handle, first, _ptr(s), sb, n, count, _ptr(out)))
+        return out
+
 
 _Q = {(32,): 0x30644e72e131a029b85045b68181585d97816a916871ca8d3c208c16d87cfd47,
       (48,): 0x1a0111ea397fe69a4b1ba7b6434bacd764774b84f38512bf6730d2a0f6b0f6241eabfffeb153ffffb9feffffffffaaab}

@@ -140,6 +140,34 @@ class ProvingKey:
         self.curve.check(self.curve.lib.sb_groth16_prove(self.curve.handle, self.handle, _ptr(w), w.size // 32, bytes(r), bytes(s), _ptr(out)))
         return out.tobytes()
 
+    def prove_batch_raw(self, witnesses, rs) -> list:
+        """witnesses = a sequence of section-2 payloads (nVars * 32 bytes each) or one buffer of them back to back;
+        rs = [(r, s), ...] one pair per witness -> affine proof bytes per witness, each equal to prove_raw's."""
+        count = len(rs)
+        if isinstance(witnesses, (list, tuple)):
+            if len(witnesses) != count:
+                raise SbError(f"{len(witnesses)} witnesses but {count} (r, s) pairs")
+            parts = [_arr(x) for x in witnesses]
+            for x in parts:
+                if x.size != 32 * self.nVars:
+                    raise SbError(f"Invalid witness length. Circuit: {self.nVars}, witness: {x.size // 32}")
+            w = np.concatenate(parts) if parts else np.zeros(0, np.uint8)
+        else:
+            w = _arr(witnesses)
+            if w.size != 32 * self.nVars * count:
+                raise SbError(f"{w.size} witness bytes are not {count} witnesses of {self.nVars} elements")
+        if count == 0:
+            return []
+        r = np.frombuffer(b"".join(bytes(x[0]) for x in rs), np.uint8)
+        s = np.frombuffer(b"".join(bytes(x[1]) for x in rs), np.uint8)
+        if r.size != 32 * count or s.size != 32 * count:
+            raise SbError("r and s must be 32-byte Fr elements")
+        pb = 8 * self.curve.n8q
+        out = np.empty(count * pb, np.uint8)
+        self.curve.check(self.curve.lib.sb_groth16_prove_batch(self.curve.handle, self.handle, _ptr(w), w.size // 32 // count, count,
+                                                               _ptr(r), _ptr(s), _ptr(out)))
+        return [out[i * pb:(i + 1) * pb].tobytes() for i in range(count)]
+
     def prove_shard(self, witness, shard: int, n_shards: int) -> np.ndarray:
         w = _arr(witness)
         out = np.empty(self.curve.lib.sb_groth16_partials_bytes(self.curve.handle), np.uint8)
@@ -184,6 +212,35 @@ def prove(zkey, wtns: bytes, r: bytes | None = None, s: bytes | None = None, log
         aff = pk.prove_raw(np.frombuffer(W, np.uint8), r, s)
         pub = [str(int.from_bytes(W[i * 32:(i + 1) * 32], "little")) for i in range(1, pk.nPublic + 1)]
         return proof_to_object(pk.curve, aff), pub
+    finally:
+        if not isinstance(zkey, ProvingKey):
+            pk.release()
+
+
+def prove_batch(zkey, wtns_list, rs=None):
+    """groth16Prove over many witnesses of one circuit in one device call: [(proof, publicSignals), ...] in the order of
+    wtns_list.  zkey may be bytes or a ProvingKey; every .wtns container is checked as prove checks it (curve, nWitness);
+    rs = [(r, s), ...] (32-byte Montgomery Fr), drawn like Fr.random() when not given."""
+    pk = zkey if isinstance(zkey, ProvingKey) else ProvingKey(zkey)
+    try:
+        ws = []
+        for wtns in wtns_list:
+            wh, W = read_wtns_header(bytes(wtns))
+            if wh["q"] != pk.header["r"]:
+                raise SbError("Curve of the witness does not match the curve of the proving key")
+            if wh["nWitness"] != pk.nVars:
+                raise SbError(f"Invalid witness length. Circuit: {pk.nVars}, witness: {wh['nWitness']}")
+            ws.append(W)
+        if rs is None:
+            rs = [(random_fr(pk.curve), random_fr(pk.curve)) for _ in ws]
+        if len(rs) != len(ws):
+            raise SbError("one (r, s) pair per witness")
+        affs = pk.prove_batch_raw([np.frombuffer(W, np.uint8) for W in ws], rs)
+        out = []
+        for W, aff in zip(ws, affs):
+            pub = [str(int.from_bytes(W[i * 32:(i + 1) * 32], "little")) for i in range(1, pk.nPublic + 1)]
+            out.append((proof_to_object(pk.curve, aff), pub))
+        return out
     finally:
         if not isinstance(zkey, ProvingKey):
             pk.release()
