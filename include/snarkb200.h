@@ -145,6 +145,22 @@ uint32_t sb_plonk_proof_bytes(sb_ctx* ctx);
 int sb_plonk_prove_resident(sb_ctx* ctx, uint64_t handle, const uint8_t* blinders, uint8_t* proof_out);
 int sb_plonk_prove(sb_ctx* ctx, uint64_t handle, const uint8_t* witness, uint64_t n_witness, const uint8_t* blinders,
                    uint8_t* proof_out);
+/* count PLONK proofs against one loaded key.  witnesses = count * n_witness * 32 bytes (wtns section-2 payloads, back to
+ * back, n_witness = nVars - nAdditions); blinders = count * 11 * 32 bytes (b_1..b_11 per proof, Montgomery);
+ * proofs_out = count * sb_plonk_proof_bytes(); status_out = count int32 (may be NULL).
+ * Proof k is byte-identical to sb_plonk_prove(witness k, blinders k).  The proofs run in lockstep in sub-batches sized from
+ * free device memory (sb_set_tuning(14) caps them): each round's kernels, NTTs and commitments run once over a sub-batch.
+ * - Argument errors come before any device work: a wrong n_witness gives "Invalid witness length. Circuit: N, witness: M, A";
+ *   an invalid handle or a null pointer gives SB_ERR_ARG; count == 0 writes nothing and returns SB_OK.
+ * - A proof the reference would reject does not stop the others.  Its slot is zero-filled and status_out[k] holds the code of
+ *   its first error: 3 "Copy constraints does not match", 4 "Polynomial is not divisible", 5 "T Polynomial is not well
+ *   calculated"; 0 for a good proof.  The call then returns SB_ERR_ARG, and sb_last_error holds the text of the
+ *   lowest-index failing proof.
+ * - The batch's device buffers grow with the largest sub-batch and belong to the key (sb_plonk_release frees them).  When
+ *   not even one proof fits, the call fails with SB_ERR_NOMEM.
+ * - The resident witness of sb_plonk_prove_resident is left as it was.  sb_last_ms(0) = the whole call. */
+int sb_plonk_prove_batch(sb_ctx* ctx, uint64_t handle, const uint8_t* witnesses, uint64_t n_witness, uint32_t count,
+                         const uint8_t* blinders, uint8_t* proofs_out, int32_t* status_out);
 int sb_plonk_release(sb_ctx* ctx, uint64_t handle);
 /* ---- fflonk (src/fflonk_prove.js:51-1286), BN254 only like the reference's setup constants ----------------------
  * sb_fflonk_load: an fflonk zkey (protocol id 10, sections 2-17: src/zkey_utils.js:301-339, src/fflonk_constants.js).
@@ -238,7 +254,8 @@ double sb_calibrate(sb_ctx* ctx, int what);
  *      is chosen: per chunk for MSMs on unregistered bases, and for window tables when they are built, i.e. when bases are
  *      registered or a key is loaded; a table keeps the c in force at that moment.  Tables are still skipped when
  *      W * n >= 2^31.  A large c costs memory: a plain MSM allocates W * 2^(c-1) buckets.
- *  14  most proofs per sub-batch of sb_groth16_prove_batch, and rows per sub-batch of sb_msm_registered_batch (test hook;
+ *  14  most proofs per sub-batch of sb_groth16_prove_batch and sb_plonk_prove_batch, and rows per sub-batch of
+ *      sb_msm_registered_batch (test hook;
  *      0 = default: as many as the 32-bit bucket keys and free device memory allow)
  * The Python mirror applies SB_TUNE="key=value,..." from the environment when it loads the library. */
 int sb_set_tuning(int key, int value);

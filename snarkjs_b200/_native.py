@@ -55,6 +55,7 @@ _SIGNATURES = {
     "sb_plonk_info": (ctypes.c_int, [vp, u64, ctypes.POINTER(u32), ctypes.POINTER(u32), ctypes.POINTER(u32), ctypes.POINTER(u32)]),
     "sb_plonk_proof_bytes": (u32, [vp]),
     "sb_plonk_prove": (ctypes.c_int, [vp, u64, vp, u64, ctypes.c_char_p, vp]),
+    "sb_plonk_prove_batch": (ctypes.c_int, [vp, u64, vp, u64, u32, vp, vp, vp]),
     "sb_plonk_prove_resident": (ctypes.c_int, [vp, u64, ctypes.c_char_p, vp]),
     "sb_plonk_release": (ctypes.c_int, [vp, u64]),
     "sb_fflonk_load": (ctypes.c_int, [vp, vp, u64, ctypes.POINTER(u64)]),

@@ -642,6 +642,36 @@ static uint32_t batch_size(sb_ctx* c, uint32_t count, uint64_t key_limit, size_t
     return (uint32_t)std::max<uint64_t>(kb, 1);
 }
 
+// rows MSMs of n scalars each over one base set (row q's scalars at d_sc + q * n * sb, on the device), sorted and reduced
+// together: one sort with MsmGeom::K = rows, one bucket pipeline, one download of the window sums, and each row recombined
+// on its own into out (rows x XYZZ).  g is the set's geometry (table mode: the table's, with first and W set); rows must
+// not exceed msm_batch_limit, and n one MSM chunk.
+static int msm_rows_dev(sb_ctx* c, const GroupOps& G, const void* d_bases, const MsmGeom& g, const uint8_t* d_sc, uint32_t sb, uint64_t n,
+                        uint32_t rows, uint8_t* out) {
+    const size_t wrow = (size_t)msm_wsum_parts(g) * g.windows_per_proof() * G.xyzz_bytes;   // window-sum bytes of one row
+    MsmGeom gK = g; gK.K = rows;
+    void* d_wsum = c->io[3].get(rows * wrow);
+    if (!d_wsum) return fail(c, SB_ERR_NOMEM, "out of device memory");
+    MsmSorted srt;
+    int rc = msm_sort_entries(d_sc, sb, n, gK, c->sort_scratch, c->stream, &srt, &c->stats);
+    if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
+    c->stats.cur_tag = (&G == &c->g1) ? SB_G1 : SB_G2;
+    rc = G.buckets(d_bases, srt, c->bucket_scratch, c->stream, d_wsum, &c->stats, nullptr, nullptr);
+    if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_buckets");
+    std::vector<uint8_t> ws(rows * wrow);
+    uint64_t entries = 0;
+    CU(c, cudaMemcpyAsync(ws.data(), d_wsum, ws.size(), cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaMemcpyAsync(&entries, srt.counts, 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    c->stat[(&G == &c->g1) ? 4 : 5] += (double)entries;
+    for (uint32_t q = 0; q < rows; q++) {
+        uint8_t* acc = out + (size_t)q * G.xyzz_bytes;
+        memset(acc, 0, G.xyzz_bytes);
+        G.combine(ws.data() + q * wrow, g, acc);
+    }
+    return 0;
+}
+
 // count MSMs over the same registered bases: the rows are sorted and reduced together in sub-batches (MsmGeom::K), each row
 // recombined on its own.  Rows longer than an MSM chunk (2^23 points) go one by one through sb_msm_registered's path.
 int sb_msm_registered_batch(sb_ctx* c, uint64_t h, uint64_t first, const uint8_t* scalars, uint32_t sb, uint64_t n, uint32_t count, uint8_t* out) { SB_LOCK(c);
@@ -670,33 +700,17 @@ int sb_msm_registered_batch(sb_ctx* c, uint64_t h, uint64_t first, const uint8_t
     const uint64_t e = n * (uint64_t)g.W;
     const size_t per_row = (size_t)n * sb + sort_batch_bytes(e) + msm_batch_bytes(e, (uint64_t)g.windows_per_proof() * g.B, G.xyzz_bytes);
     const uint32_t KB = batch_size(c, count, msm_batch_limit(n, g.c, g.W, g.precomp), per_row, c->io[1].cap + c->io[3].cap);
-    const size_t wrow = (size_t)msm_wsum_parts(g) * g.windows_per_proof() * G.xyzz_bytes;   // window-sum bytes of one row
+    std::vector<uint8_t> sums((size_t)KB * G.xyzz_bytes);
     tick(c, 0);
     prof_begin(c);
     for (uint32_t r0 = 0; r0 < count; r0 += KB) {
         const uint32_t kb = std::min(KB, count - r0);
-        MsmGeom gK = g; gK.K = kb;
         uint8_t* d_sc = (uint8_t*)c->io[1].get((size_t)kb * n * sb);
-        void* d_wsum = c->io[3].get(kb * wrow);
-        if (!d_sc || !d_wsum) return fail(c, SB_ERR_NOMEM, "out of device memory");
+        if (!d_sc) return fail(c, SB_ERR_NOMEM, "out of device memory");
         CU(c, h2d(c, d_sc, scalars + (size_t)r0 * n * sb, (size_t)kb * n * sb));
-        MsmSorted srt;
-        int rc = msm_sort_entries(d_sc, sb, n, gK, c->sort_scratch, c->stream, &srt, &c->stats);
-        if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
-        c->stats.cur_tag = (&G == &c->g1) ? SB_G1 : SB_G2;
-        rc = G.buckets(d_bases, srt, c->bucket_scratch, c->stream, d_wsum, &c->stats, nullptr, nullptr);
-        if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_buckets");
-        std::vector<uint8_t> ws(kb * wrow);
-        uint64_t entries = 0;
-        CU(c, cudaMemcpyAsync(ws.data(), d_wsum, ws.size(), cudaMemcpyDeviceToHost, c->stream));
-        CU(c, cudaMemcpyAsync(&entries, srt.counts, 8, cudaMemcpyDeviceToHost, c->stream));
-        CU(c, cudaStreamSynchronize(c->stream));
-        c->stat[(&G == &c->g1) ? 4 : 5] += (double)entries;
-        for (uint32_t q = 0; q < kb; q++) {
-            std::fill(acc.begin(), acc.end(), 0);
-            G.combine(ws.data() + q * wrow, g, acc.data());
-            G.to_jacobian(acc.data(), out + (size_t)(r0 + q) * jb);
-        }
+        int rc = msm_rows_dev(c, G, d_bases, g, d_sc, sb, n, kb, sums.data());
+        if (rc) return rc;
+        for (uint32_t q = 0; q < kb; q++) G.to_jacobian(sums.data() + (size_t)q * G.xyzz_bytes, out + (size_t)(r0 + q) * jb);
     }
     tick(c, 1);
     CU(c, cudaEventSynchronize(c->ev[1]));
@@ -1859,6 +1873,17 @@ int sb_plonk_prove_resident(sb_ctx* c, uint64_t h, const uint8_t* blinders, uint
     cudaSetDevice(c->device);
     return c->curve == SB_BN254 ? plonk_prove_impl<BnFq, BnFr>(c, k, nullptr, 0, blinders, proof)
                                 : plonk_prove_impl<BlsFq, BlsFr>(c, k, nullptr, 0, blinders, proof);
+}
+int sb_plonk_prove_batch(sb_ctx* c, uint64_t h, const uint8_t* witnesses, uint64_t n_witness, uint32_t count, const uint8_t* blinders,
+                         uint8_t* proofs, int32_t* status) { SB_LOCK(c);
+    PlonkKeyDev* k = get_plonk_key(c, h); if (!k) return fail(c, SB_ERR_ARG, "invalid plonk handle");
+    if (n_witness != (uint64_t)k->z.nVars - k->z.nAdditions)                                          // plonk_prove.js:66-68
+        return fail(c, SB_ERR_ARG, "Invalid witness length. Circuit: " + std::to_string(k->z.nVars) + ", witness: " + std::to_string(n_witness) + ", " + std::to_string(k->z.nAdditions));
+    if (count == 0) return SB_OK;
+    if (!witnesses || !blinders || !proofs) return fail(c, SB_ERR_ARG, "null argument");
+    cudaSetDevice(c->device);
+    return c->curve == SB_BN254 ? plonk_prove_batch_impl<BnFq, BnFr>(c, k, witnesses, n_witness, count, blinders, proofs, status)
+                                : plonk_prove_batch_impl<BlsFq, BlsFr>(c, k, witnesses, n_witness, count, blinders, proofs, status);
 }
 int sb_plonk_release(sb_ctx* c, uint64_t h) { SB_LOCK(c);
     PlonkKeyDev* k = get_plonk_key(c, h); if (!k) return fail(c, SB_ERR_ARG, "invalid plonk handle");

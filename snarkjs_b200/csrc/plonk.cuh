@@ -53,6 +53,13 @@ template <class F> SB_HD void pl_st(F* p, const F& x) {
 template <class F> SB_HD F pl_pow(const PlonkPow<F>& t, uint64_t i) {
     return F::mul(pl_ld(t.lo + (i & ((1ull << t.h) - 1))), pl_ld(t.hi + (i >> t.h)));
 }
+// one power table per proof of a batch: proof q's tables start at lo + q * slo and hi + q * shi
+template <class F> struct PlonkPowK {
+    const F* lo = nullptr; const F* hi = nullptr; int h = 0; uint64_t slo = 0, shi = 0;
+    SB_HD PlonkPow<F> at(uint64_t q) const { PlonkPow<F> p; p.lo = lo + q * slo; p.hi = hi + q * shi; p.h = h; return p; }
+};
+// which blinders b[idx[j][0..cnt)] go onto the rows of group j (a batch blinds groups x K rows, group-major)
+struct PlonkBlindIdx { int cnt; int idx[3][3]; };
 
 // ---------------------------------------------------------------------------------------------- round 1
 // calculateAdditions (plonk_prove.js:166-195): w[n_wit + i] = f1 * w[s1] + f2 * w[s2].  Factors are Montgomery, the witness
@@ -301,6 +308,130 @@ template <class F> __global__ void k_pl_quot(uint64_t m, const F* P, PlonkPow<F>
     if (j == 0 && !pl_ld(P + m - 1).is_zero()) atomicOr(flag, 1);
     pl_st(q_plain + j, F::from_mont(pl_quot_coef<F>(j, m, P, ipow)));
 }
+
+// ------------------------------------------------------------------------------------------------ batched kernels
+// The kernels above with a proof axis (blockIdx.y = proof q, or row of a group-major array): every work array holds the K
+// proofs back to back at a fixed stride, and per-proof scalars (PlonkRound, PlonkLin, power tables) come from small device
+// arrays indexed by the proof.  A block never spans two proofs, so a block stages its proof's scalars in shared memory once.
+template <class T> __device__ __forceinline__ const T& pl_stage(uint32_t* sh, const T* src) {
+    const uint32_t* s = reinterpret_cast<const uint32_t*>(src);
+    for (unsigned t = threadIdx.x; t < sizeof(T) / 4; t += blockDim.x) sh[t] = s[t];
+    __syncthreads();
+    return *reinterpret_cast<const T*>(sh);
+}
+template <class F> __global__ void k_plb_additions(const uint32_t* __restrict__ order, uint32_t lo, uint32_t hi, const uint32_t* __restrict__ sig,
+                                                   const F* __restrict__ fac, F* w, uint64_t sw, uint32_t n_wit, uint32_t n_vars) {
+    uint32_t j = lo + blockIdx.x * blockDim.x + threadIdx.x;
+    if (j < hi) pl_addition<F>(order[j], sig, fac, w + blockIdx.y * sw, n_wit, n_vars);
+}
+// grid (., K, 3): wire j of proof q goes to row j K + q of out (rows of n)
+template <class F> __global__ void k_plb_wires(PlonkMaps mp, const F* __restrict__ w, uint64_t sw, uint32_t n_vars, uint64_t n_cons, uint64_t n, F* out) {
+    uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (i < n) pl_wire<F>(i, mp.m[blockIdx.z], w + blockIdx.y * sw, n_vars, n_cons, out + ((uint64_t)blockIdx.z * gridDim.y + blockIdx.y) * n);
+}
+// one thread per row of groups x K rows of `stride` elements
+template <class F> __global__ void k_plb_blind(F* p, uint64_t stride, uint64_t n, uint32_t rows, uint32_t K, const PlonkRound<F>* rs, PlonkBlindIdx bi) {
+    uint32_t row = blockIdx.x * blockDim.x + threadIdx.x;
+    if (row >= rows) return;
+    const uint32_t j = row / K, q = row % K;
+    F bf[3];
+    for (int t = 0; t < bi.cnt; t++) bf[t] = pl_ld(&rs[q].b[bi.idx[j][t]]);
+    pl_blind<F>(p + row * stride, n, bf, bi.cnt);
+}
+// wires: 3K rows of n (A rows, then B, then C)
+template <class F> __global__ void __launch_bounds__(128) k_plb_z_terms(uint64_t n, const F* wires, const F* s1, const F* s2, const F* s3,
+                                                                        PlonkPow<F> wpow, const PlonkRound<F>* rs, F* num, F* den) {
+    __shared__ __align__(16) uint32_t sh[sizeof(PlonkRound<F>) / 4];
+    const uint64_t q = blockIdx.y, K = gridDim.y;
+    const PlonkRound<F>& r = pl_stage(sh, rs + q);
+    uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (i < n) pl_z_terms<F>(i, wires + q * n, wires + (K + q) * n, wires + (2 * K + q) * n, s1, s2, s3, wpow, r, num + q * n, den + q * n);
+}
+// one thread per proof: flag[q] |= 4 unless z[n-1] * ratio[n-1] == 1 in proof q's rows
+template <class F> __global__ void k_plb_z_check(const F* z, const F* ratio, uint64_t n, uint32_t K, int* flag) {
+    uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= K) return;
+    F t = F::mul(pl_ld(z + q * n + n - 1), pl_ld(ratio + q * n + n - 1));
+    if (!(t == F::one())) flag[q] |= 4;
+}
+// ev: 3K rows of 4n (A, B, C evaluations), evZ: K rows of 4n, wires: A's rows give the public inputs; T, Tz: K rows of 4n
+template <class F> __global__ void __launch_bounds__(128) k_plb_t(uint64_t n4, uint64_t n, PlonkTIn in, const F* ev, const F* evZ, const F* wires,
+                                                                  PlonkPow<F> w4pow, const PlonkRound<F>* rs, F* T, F* Tz) {
+    __shared__ __align__(16) uint32_t sh[sizeof(PlonkRound<F>) / 4];
+    const uint64_t q = blockIdx.y, K = gridDim.y;
+    const PlonkRound<F>& r = pl_stage(sh, rs + q);
+    uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (i >= n4) return;
+    in.A = ev + q * n4; in.B = ev + (K + q) * n4; in.C = ev + (2 * K + q) * n4; in.Z = evZ + q * n4; in.pubA = wires + q * n;
+    pl_t_eval<F>(i, n4, in, w4pow, r, T + q * n4, Tz + q * n4);
+}
+// t: T rows then Tz rows (K each, 4n); out: K rows of 4n
+template <class F> __global__ void k_plb_divzh(uint64_t n, const F* t, F* out, int* flag) {
+    const uint64_t q = blockIdx.y, K = gridDim.y, n4 = 4 * n;
+    uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (i < n) { int bad = pl_divzh<F>(i, n, t + q * n4, t + (K + q) * n4, out + q * n4); if (bad) atomicOr(flag + q, bad); }
+}
+// cT: 3K rows of stride p (T1 rows, T2 rows, T3 rows)
+template <class F> __global__ void k_plb_tsplit(uint64_t n, uint64_t p, const F* t, const PlonkRound<F>* rs, F* cT) {
+    const uint64_t q = blockIdx.y, K = gridDim.y;
+    uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (i < n + 6) pl_tsplit<F>(i, n, t + q * 4 * n, pl_ld(&rs[q].b[10]), pl_ld(&rs[q].b[11]), cT + q * p, cT + (K + q) * p, cT + (2 * K + q) * p);
+}
+// round 4's six evaluations of every proof: row 6q + e of g (stride p) holds f_e[i] x^i, zero from the polynomial's length on.
+// e = A, B, C (n + 2 coefficients), S1, S2 (n, the key's), Z (n + 3, at xi w); cABC: 3K rows, cZ: K rows, stride p.
+template <class F> __global__ void k_plb_eval_terms(uint64_t n, uint64_t p, const F* cABC, const F* s1, const F* s2, const F* cZ,
+                                                    PlonkPowK<F> pxi, PlonkPowK<F> pxiw, F* g) {
+    const uint64_t row = blockIdx.y, q = row / 6, K = gridDim.y / 6; const int e = (int)(row % 6);
+    uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (i >= p) return;
+    const F* f; uint64_t len = n;
+    if (e < 3) { f = cABC + (e * K + q) * p; len = n + 2; }
+    else if (e == 3) f = s1;
+    else if (e == 4) f = s2;
+    else { f = cZ + q * p; len = n + 3; }
+    pl_st(g + row * p + i, i < len ? F::mul(pl_ld(f + i), pl_pow(e == 5 ? pxiw.at(q) : pxi.at(q), i)) : F::zero());
+}
+// round 5's two divisions of every proof: row q of g (stride p = n + 6) is Wxi's numerator (computeR + computeWxi) times
+// xi^i, row K + q is (Z - eval_zw) times (xi w)^i for i < n + 3 and zero after.  kin: the key's coefficient arrays.
+template <class F> __global__ void __launch_bounds__(128) k_plb_wxi(uint64_t n, uint64_t p, PlonkLinIn kin, const F* cABC, const F* cZ, const F* cT,
+                                                                    const PlonkLin<F>* Ls, const F* ezw, PlonkPowK<F> pxi, PlonkPowK<F> pxiw, F* g) {
+    __shared__ __align__(16) uint32_t sh[sizeof(PlonkLin<F>) / 4];
+    const uint64_t K = gridDim.y / 2, row = blockIdx.y, q = row % K;
+    uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (row < K) {
+        const PlonkLin<F>& L = pl_stage(sh, Ls + q);
+        if (i >= p) return;
+        kin.A = cABC + q * p; kin.B = cABC + (K + q) * p; kin.C = cABC + (2 * K + q) * p; kin.Z = cZ + q * p;
+        kin.T1 = cT + q * p; kin.T2 = cT + (K + q) * p; kin.T3 = cT + (2 * K + q) * p;
+        pl_st(g + row * p + i, F::mul(pl_wxi_coef<F>(i, n, kin, L), pl_pow(pxi.at(q), i)));
+    } else {
+        if (i >= p) return;
+        F x = i < n + 3 ? pl_ld(cZ + q * p + i) : F::zero();
+        if (i == 0) x = F::sub(x, pl_ld(ezw + q));
+        pl_st(g + row * p + i, F::mul(x, pl_pow(pxiw.at(q), i)));
+    }
+}
+// quotient rows from their inclusive sums P (stride p): row q divides by X - xi (m = n + 6), row K + q by X - xi w (m = n + 3);
+// plain scalars, zero from m on; flag[q] |= 1 when a remainder is not zero
+template <class F> __global__ void k_plb_quot(uint64_t n, uint64_t p, const F* P, PlonkPowK<F> ipxi, PlonkPowK<F> ipxiw, F* q_plain, int* flag) {
+    const uint64_t K = gridDim.y / 2, row = blockIdx.y, q = row % K;
+    const uint64_t m = row < K ? n + 6 : n + 3;
+    uint64_t j = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
+    if (j >= p) return;
+    const F* Pr = P + row * p;
+    if (j == 0 && !pl_ld(Pr + m - 1).is_zero()) atomicOr(flag + q, 1);
+    pl_st(q_plain + row * p + j, j < m ? F::from_mont(pl_quot_coef<F>(j, m, Pr, row < K ? ipxi.at(q) : ipxiw.at(q))) : F::zero());
+}
+// segment id of an array-major batch: element idx belongs to row idx / len
+struct PlbRowKey {
+    uint64_t len;
+    __host__ __device__ __forceinline__ uint32_t operator()(uint64_t idx) const { return (uint32_t)(idx / len); }
+};
+struct PlbRowOff {
+    uint64_t len;
+    __host__ __device__ __forceinline__ int64_t operator()(uint64_t row) const { return (int64_t)(row * len); }
+};
+
 struct FrAddOp { template <class F> __host__ __device__ __forceinline__ F operator()(const F& a, const F& b) const { return F::add(a, b); } };
 struct FrMulOp { template <class F> __host__ __device__ __forceinline__ F operator()(const F& a, const F& b) const { return F::mul(a, b); } };
 #endif  // __CUDACC__
