@@ -134,7 +134,10 @@ int sb_groth16_release(sb_ctx* ctx, uint64_t handle);
  *   proof_out = A B C Z T1 T2 T3 Wxi Wxiw (affine Montgomery, 2*n8q bytes each) then eval_a eval_b eval_c eval_s1
  *   eval_s2 eval_zw (Montgomery, 32 bytes each): sb_plonk_proof_bytes().  Errors carry the reference's texts:
  *   "Invalid witness length. Circuit: N, witness: M, A", "Copy constraints does not match" (:436-438),
- *   "Polynomial is not divisible" (polynomial.js:608, 653), "T Polynomial is not well calculated" (:648-650). */
+ *   "Polynomial is not divisible" (polynomial.js:608, 653), "T Polynomial is not well calculated" (:648-650), and for a key
+ *   with nPublic = 0, "Evaluations.getEvaluation() out of bounds" (round 3, :613-617, where the reference reads L1 from an
+ *   empty Lagrange buffer).  A witness refused at round 2 or later stays resident, so sb_plonk_prove_resident refuses it
+ *   with the same text. */
 int sb_plonk_load(sb_ctx* ctx, const uint8_t* zkey, uint64_t zkey_len, uint64_t* handle);
 /* same from a file: the .zkey is mapped read-only and streamed to HBM section by section (SURVEY §8f rank 2) */
 int sb_plonk_load_file(sb_ctx* ctx, const char* zkey_path, uint64_t* handle);
@@ -154,7 +157,8 @@ int sb_plonk_prove(sb_ctx* ctx, uint64_t handle, const uint8_t* witness, uint64_
  *   an invalid handle or a null pointer gives SB_ERR_ARG; count == 0 writes nothing and returns SB_OK.
  * - A proof the reference would reject does not stop the others.  Its slot is zero-filled and status_out[k] holds the code of
  *   its first error: 3 "Copy constraints does not match", 4 "Polynomial is not divisible", 5 "T Polynomial is not well
- *   calculated"; 0 for a good proof.  The call then returns SB_ERR_ARG, and sb_last_error holds the text of the
+ *   calculated", 6 "Evaluations.getEvaluation() out of bounds" (every proof not refused earlier, on a key with nPublic = 0);
+ *   0 for a good proof.  The call then returns SB_ERR_ARG, and sb_last_error holds the text of the
  *   lowest-index failing proof.
  * - The batch's device buffers grow with the largest sub-batch and belong to the key (sb_plonk_release frees them).  When
  *   not even one proof fits, the call fails with SB_ERR_NOMEM.

@@ -462,7 +462,9 @@ def plonk_prove(zkey, wtns, blinders: Sequence[int], return_parts: bool = False)
     t.reset(); t.add_scalar(beta); t.add_scalar(gamma); t.add_pol(proof_pts["Z"])
     alpha = t.challenge()
     alpha2 = alpha * alpha % r
-    q_ev = {name: sec_ints(sid, n, 4 * n) for name, sid in (("QM", 7), ("QL", 8), ("QR", 9), ("QO", 10), ("QC", 11))}
+    if n_pub == 0:              # e4 reads L1 from a buffer of nPublic Lagrange polynomials (:503-509, 613-617; evaluations.js:39-44)
+        raise ValueError("Evaluations.getEvaluation() out of bounds")
+    q_ev ={name: sec_ints(sid, n, 4 * n) for name, sid in (("QM", 7), ("QL", 8), ("QR", 9), ("QO", 10), ("QC", 11))}
     lag_ev = [sec_ints(13, 5 * j * n + n, 4 * n) for j in range(n_pub)]                           # :503-509
     Z1, Z2, Z3 = _mulz_consts(ci)
     w4n = _fr_w(ci, power + 2)

@@ -148,9 +148,10 @@ template <class F> inline int plonk_witness_length(const PlonkKeyView<F>& k, uin
     err = "Invalid witness length. Circuit: " + std::to_string(k.nVars) + ", witness: " + std::to_string(n_witness) + ", " + std::to_string(k.nAdditions);
     return 2;
 }
-// the reference's text for the flow's positive codes 3..5
+// the reference's text for the flow's positive codes 3..6
 inline const char* plonk_error_text(int code) {
-    return code == 3 ? "Copy constraints does not match" : code == 4 ? "Polynomial is not divisible" : code == 5 ? "T Polynomial is not well calculated" : "";
+    return code == 3 ? "Copy constraints does not match" : code == 4 ? "Polynomial is not divisible" : code == 5 ? "T Polynomial is not well calculated"
+         : code == 6 ? "Evaluations.getEvaluation() out of bounds" : "";
 }
 // round 2 (:315-330): beta, gamma from the key's eight points, the public A values and the commitments A, B, C
 template <class PQ, class PR> inline void plonk_beta_gamma(const PlonkKeyView<Fp<PR>>& k, const Fp<PR>* pubA, const uint8_t* pt_A, const uint8_t* pt_B,
@@ -232,8 +233,8 @@ template <class PQ, class PR> inline void plonk_lin(const PlonkKeyView<Fp<PR>>& 
 //   int quotient(const F* f_or_null, const PlonkLinIn*, const PlonkLin<F>*, uint64_t n, uint64_t len, uint64_t m, const F& sub0,
 //                const PlonkPow<F>& pw, const PlonkPow<F>& ipw, F* g, F* P, F* q_plain); // f / (X - b) -> plain scalars
 //   int commit_plain(const F* scal_plain, uint64_t len, uint8_t* affine);
-// Returns 0, a positive code for the reference's own errors (2 witness length, 3 copy constraints, 4 divisibility; err holds
-// the reference's message) or the backend's negative code.
+// Returns 0, a positive code for the reference's own errors (2 witness length, 3 copy constraints, 4 divisibility, 6 a key
+// without public signals; err holds the reference's message) or the backend's negative code.
 template <class PQ, class PR, class B>
 int plonk_prove_flow(B& be, const PlonkKeyView<Fp<PR>>& k, PlonkWork<Fp<PR>>& w, const uint8_t* witness_plain, uint64_t n_witness,
                      const uint8_t* blinders_mont /*11 x 32*/, uint8_t* proof_out, std::string& err) {
@@ -290,6 +291,9 @@ int plonk_prove_flow(B& be, const PlonkKeyView<Fp<PR>>& k, PlonkWork<Fp<PR>>& w,
     }
     be.mark(2);
     // ---------------- round 3 (:460-684)
+    // e4 reads L1 from a buffer of nPublic Lagrange polynomials (:503-509), which throws on a key without public signals
+    // (:613-617, evaluations.js:39-44)
+    if (!k.nPublic) { err = plonk_error_text(6); return 6; }
     plonk_alpha<PQ, PR>(pt_Z, r);
     {
         be.t(k, r, w);
@@ -375,7 +379,7 @@ template <class F> struct PlonkBatchWork {        // backend memory, F elements;
 //   void evals(const PlonkKeyView<F>&, const PlonkBatchWork<F>&, const PlonkPowK<F>& pxi, const PlonkPowK<F>& pxiw, uint32_t K, F* out /*K x 6*/);
 //   void quotients(const PlonkKeyView<F>&, const PlonkBatchWork<F>&, const PlonkPowK<F> pw[4], uint32_t K, int* flags);   // -> 2K rows of w.scal
 //   int commit(const F* coef, uint32_t rows, F* scal, uint8_t* affine);  int commit_plain(const F* scal, uint32_t rows, uint8_t* affine);
-// flags (host, K ints): what the proof's step found, as the single flow's flags.  status[q] = 0 or the first code 3..5 of
+// flags (host, K ints): what the proof's step found, as the single flow's flags.  status[q] = 0 or the first code 3..6 of
 // proof q (plonk_error_text); a failing proof runs on with the others and its slot is zero-filled at the end.  Returns 0 or
 // the backend's negative code.  The caller checks the witness length.
 template <class PQ, class PR, class BB>
@@ -435,6 +439,11 @@ int plonk_prove_flow_batch(BB& be, const PlonkKeyView<Fp<PR>>& k, const PlonkBat
     { int rc = be.commit(w.cZ, K, w.scal, pts.data()); if (rc) return rc; }
     scatter(1, 3);
     // ---------------- round 3
+    if (!k.nPublic) {                                                                                // as the single flow: code 6
+        for (uint32_t q = 0; q < K; q++) if (!status[q]) status[q] = 6;
+        memset(proofs_out, 0, K * pb);
+        return 0;
+    }
     for (uint32_t q = 0; q < K; q++) plonk_alpha<PQ, PR>(pt(q, 3), r[q]);
     be.set_rounds(r.data(), K);
     be.t(k, ev, w.evZ, w.wires, fr, K);                                                              // T rows, then Tz rows

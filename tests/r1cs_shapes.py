@@ -9,6 +9,7 @@ nVars equal to the domain.  The classes here vary what that chain keeps fixed:
   empty   constraints with an empty A side, an empty B side, both, or all three
   public  nPublic public signals, split between outputs and public inputs, each one used by a constraint
   fit     nConstraints + nPublic + 1 exactly 2^k (no zero rows), or 2^k + 1 (the domain doubles)
+  gates   the same for PLONK and fflonk keys: exactly 2^k + extra gates, with no additions
   ratio   nVars far above or far below the domain, so that the witness MSMs and the H MSM get different geometries
   tiny    a given nVars, down to 1; nVars = nPublic + 1 leaves no private signal and an empty section 8
 
@@ -23,7 +24,9 @@ Keys come two ways:
   unstructured_zkey  the key's header and section 4 exactly as zkey_new writes them, with random valid curve points as
                      bases (the layout of snarkjs_b200.synth.groth16_zkey_image): proofs do not verify, but the bytes
                      of every proof are defined.  For any size.
-shuffle() permutes the section 4 entries; the prover sums a row's entries in any order, so proofs must not change."""
+shuffle() permutes the section 4 entries; the prover sums a row's entries in any order, so proofs must not change.
+PLONK and fflonk keys (PLONK_CASES) come from oracle.plonk.plonk_setup / oracle.fflonk.fflonk_setup over a ptau with the
+same known tau (oracle.synth_setup.plonk_ptau), or with pseudo-random points in place of its powers."""
 from __future__ import annotations
 
 import functools
@@ -194,7 +197,9 @@ class Wide(Circuit):
 
 class Coeffs(Circuit):
     """Coefficients at the edges of Fr, explicit zero entries, a signal twice in one linear combination, and the
-    constant signal with large coefficients."""
+    constant signal with large coefficients.  repeat=False keeps every signal to one entry per linear combination: PLONK
+    and fflonk keys key a linear combination by signal, so a repeated signal's last entry overwrites the others and the
+    key no longer encodes the circuit (src/plonk_setup.js, src/r1cs_constraint_processor.js)."""
     name = "coeffs"
 
     def coef(self):
@@ -205,16 +210,23 @@ class Coeffs(Circuit):
     def lc(self, pool, k):
         out = [(self.rnd.choice(pool), self.coef()) for _ in range(k)]
         if out and self.rnd.random() < 0.5:                 # the same signal twice: the entries must add up
-            s = out[0][0]
-            out.append((s, self.coef()))
+            s, v = out[0][0], self.coef()
+            if self.repeat:
+                out.append((s, v))
         if self.rnd.random() < 0.3:                         # the constant signal with a large coefficient
             out.append((0, self.r - 1 - self.rnd.randrange(1 << 32)))
         if self.rnd.random() < 0.3:                         # an explicit zero entry
             out.append((self.rnd.choice(pool), 0))
+        if not self.repeat:                                 # the first entry of each signal
+            first = {}
+            for s, v in out:
+                first.setdefault(s, v)
+            out = list(first.items())
         self.rnd.shuffle(out)
         return out
 
-    def build(self, rows=96):
+    def build(self, rows=96, repeat=True):
+        self.repeat = repeat
         x = self.new("pub")
         pool = [x] + [self.new("prv") for _ in range(12)]
         specials = [0, 1, self.r - 1, (self.r - 1) // 2, 1 << 200]
@@ -227,7 +239,7 @@ class Coeffs(Circuit):
             pool.append(self.solve(A, B, C, kind, c))
         # a row whose A and B entries all carry the coefficient 0, next to ones that cancel to zero
         z = pool[3]
-        self.add([(z, 0), (pool[4], 0)], [(z, 1)], [(z, 5), (z, self.r - 5)])
+        self.add([(z, 0), (pool[4], 0)], [(z, 1)], [(z, 5), (z, self.r - 5)] if repeat else [(z, 0), (pool[5], 0)])
 
 
 class Empty(Circuit):
@@ -289,6 +301,19 @@ class Fit(Circuit):
         self.solve([(prev[-1], 1)], [(0, 1)], [], "out")
 
 
+class Gates(Circuit):
+    """Two public inputs and 2^k + extra - 2 rows of one entry per side (no PLONK additions): 2^k + extra PLONK / fflonk
+    gates.  PLONK's domain is 2^bitlen(gates - 1) and fflonk's 2^bitlen(gates + 1), as fflonk keeps two rows for its
+    blinding: extra = 0 / 1 fills / doubles the PLONK domain, extra = -2 / -1 the fflonk domain."""
+    name = "gates"
+
+    def build(self, k=8, extra=0):
+        prev = [self.new("pub"), self.new("pub")]
+        for i in range((1 << k) + extra - 2):
+            a, b = self.rnd.randrange(1, self.r), self.rnd.randrange(1, self.r)
+            prev.append(self.solve([(prev[-1], a)], [(prev[-2], b)], [], coef=(i % 7) + 1))
+
+
 class Ratio(Circuit):
     """mode 'vars': n_vars signals in rows + 1 wide linear constraints (nVars far above the domain when rows is small);
     mode 'rows': four signals in `rows` repeated constraints (nVars far below the domain)."""
@@ -341,7 +366,7 @@ class Tiny(Circuit):
             self.add([(p[0], 1)], [(0, 1)], [(p[0], 1), (p[-1], 0)])
 
 
-SHAPES = {cls.name: cls for cls in (Bits, Wide, Coeffs, Empty, Public, Fit, Ratio, Tiny)}
+SHAPES = {cls.name: cls for cls in (Bits, Wide, Coeffs, Empty, Public, Fit, Gates, Ratio, Tiny)}
 
 BN, BLS = O.BN254, O.BLS12_381
 
@@ -371,9 +396,32 @@ CASES = {
 }
 
 
+# The same format for PLONK and fflonk keys (plonk_zkey / fflonk_zkey), with CASES' labels where the circuit is the same.
+# Structured keys are for domains of 1024 and below.  The tiny circuits give the minimum domain of 8 and domain 32 (a
+# commitment of n + 3 ... n + 6 <= 49 points takes 3-bit windows on BN254); public17 / public300 put 17 / 300 Lagrange
+# terms into PI(X); bits has a 254-term linear combination, 252 additions in a chain; coeffs_distinct takes edge
+# coefficients to the selectors (coeffs, with a repeated signal, gives a key that does not encode its circuit: "Polynomial is
+# not divisible"); gates*+0 / +1 fill / overflow the PLONK domain and gates*-2 / -1 the fflonk domain.  gates12* commit
+# over 4102 and 8198 points, the first sizes with window tables; wide4096 (8191 additions) and ratio_rows8192 have domain
+# 2^14.  fflonk is BN254 only, as the reference's setup constants.
+PLONK_CASES = {
+    **{label: CASES[label] for label in ("tiny1", "tiny2", "tiny4", "tiny7", "tiny48", "tiny64", "public0", "public2",
+                                         "public17", "public300", "empty", "bits", "coeffs")},
+    "coeffs_distinct": ("coeffs", BN, {"repeat": False}, True),
+    **{f"gates8{e:+d}": ("gates", BN, {"k": 8, "extra": e}, True) for e in (-2, -1, 0, 1)},
+    **{f"gates12{e:+d}": ("gates", BN, {"k": 12, "extra": e}, False) for e in (0, 1)},
+    "wide4096": ("wide", BN, {"terms": 1 << 12}, False),
+    "ratio_rows8192": ("ratio", BN, {"mode": "rows", "rows": 1 << 13}, False),
+    **{label: CASES[label] for label in ("bls_bits", "bls_public17", "bls_tiny362", "bls_tiny363", "bls_ratio_rows")},
+}
+# keys that no witness proves: the reference's prover throws this text in round 3 (fflonk proves the nPublic = 0 keys)
+PLONK_ERRORS = {"coeffs": "Polynomial is not divisible", **{label: "Evaluations.getEvaluation() out of bounds" for label in ("public0", "tiny1")}}
+FFLONK_ERRORS = {"coeffs": "Polynomial is not divisible"}
+
+
 @functools.lru_cache(maxsize=None)
 def case(label: str) -> Circuit:
-    shape, curve, params, _ = CASES[label]
+    shape, curve, params, _ = CASES[label] if label in CASES else PLONK_CASES[label]
     return SHAPES[shape](curve, 1, **params)
 
 
@@ -391,6 +439,33 @@ TOXIC = dict(tau=0x1234567890ABCDEF1234, alpha=0xA1FA5555, beta=0xBE7A7777)
 def prepared_ptau(curve: int, domain: int) -> bytes:
     """A prepared powers of tau for one (curve, domain), with known toxic waste; cached for the session."""
     return SS.prepared_ptau(curve, domain, **TOXIC)
+
+
+@functools.lru_cache(maxsize=None)
+def plonk_zkey(label: str) -> bytes:
+    """oracle.plonk.plonk_setup of the case's r1cs over plonk_ptau (structured or not, as PLONK_CASES says)."""
+    from oracle import plonk as OP
+    circ = case(label)
+    gates, _adds, _nv, _np = OP.plonk_gates_from_r1cs(O.read_r1cs(circ.r1cs_bytes()), circ.r)
+    power = max(3, (len(gates) - 1).bit_length())
+    return OP.plonk_setup(circ.r1cs_bytes(), _plonk_ptau(label, power, (1 << power) + 6))
+
+
+@functools.lru_cache(maxsize=None)
+def fflonk_zkey(label: str) -> bytes:
+    """oracle.fflonk.fflonk_setup of the case's r1cs over plonk_ptau (BN254 cases only)."""
+    from oracle import fflonk as OF
+    circ = case(label)
+    assert circ.curve == BN, "fflonk keys are BN254 only"
+    gates, _adds, _nv, _np = OF.fflonk_gates_from_r1cs(O.read_r1cs(circ.r1cs_bytes()), circ.r)
+    power = max(3, (len(gates) + 1).bit_length())
+    return OF.fflonk_setup(circ.r1cs_bytes(), _plonk_ptau(label, power, 9 * (1 << power) + 18))
+
+
+def _plonk_ptau(label: str, power: int, n_g1: int) -> bytes:
+    structured = PLONK_CASES[label][3]
+    assert not structured or power <= 10, "structured keys are for domains of 1024 and below"
+    return SS.plonk_ptau(case(label).curve, power, TOXIC["tau"], n_g1, structured)
 
 
 def structured_zkey(circ: Circuit) -> bytes:

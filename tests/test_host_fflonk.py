@@ -4,6 +4,7 @@ the oracle) and compared with oracle/fflonk.py proof for proof on the reference'
 import ctypes
 import json
 import os
+import re
 import struct
 import subprocess
 
@@ -12,6 +13,8 @@ import pytest
 from oracle import fflonk
 from oracle import oracle as orc
 from oracle import plonk
+
+from tests import r1cs_shapes as S
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BLINDERS = [0x5000 + 15485863 * i for i in range(9)]
@@ -57,17 +60,29 @@ def test_host_fflonk_reference_fixture(hostlib, golden):
     assert fflonk.fflonk_verify(json.loads(bytes(g["vk_json"])), public, got)
 
 
-@pytest.mark.parametrize("n_gates,n_pub,with_additions", [(13, 1, True), (120, 1, True), (29, 3, True), (60, 5, False), (500, 1, True)])
+@pytest.mark.parametrize("n_gates,n_pub,with_additions", [(13, 1, True), (120, 1, True), (29, 3, True), (60, 5, False), (500, 1, True)]
+                         + [pytest.param(label, None, None, id=label) for label, c in S.PLONK_CASES.items() if c[1] == orc.BN254])
 def test_host_fflonk_synthetic(hostlib, n_gates, n_pub, with_additions):
-    gates, adds, n_vars, n_pub, wit = plonk.chain_gates(n_gates, n_pub=n_pub, with_additions=with_additions)
-    zkey = fflonk.fflonk_setup_synth(gates, adds, n_vars, n_pub, tau=0xFACE0FF + n_gates, structured=n_gates < 200)
-    wtns = plonk.wtns_bytes(wit)
+    """Chain keys from fflonk_setup_synth; a label instead of a gate count takes the key fflonk_setup builds from a circuit
+    of tests/r1cs_shapes.py, and where the reference rejects it the flow gives the same text."""
+    if isinstance(n_gates, str):
+        circ = S.case(n_gates)
+        zkey, wtns, verify = S.fflonk_zkey(n_gates), circ.wtns(), S.PLONK_CASES[n_gates][3]
+    else:
+        gates, adds, n_vars, n_pub, wit = plonk.chain_gates(n_gates, n_pub=n_pub, with_additions=with_additions)
+        zkey = fflonk.fflonk_setup_synth(gates, adds, n_vars, n_pub, tau=0xFACE0FF + n_gates, structured=n_gates < 200)
+        wtns, verify = plonk.wtns_bytes(wit), n_gates < 200
     rc, err, raw = host_prove(hostlib, zkey, wtns, BLINDERS)
+    if n_gates in S.FFLONK_ERRORS:
+        assert rc != 0 and err == S.FFLONK_ERRORS[n_gates]
+        with pytest.raises(ValueError, match=re.escape(err)):
+            fflonk.fflonk_prove(zkey, wtns, BLINDERS)
+        return
     assert rc == 0, err
     want, public = fflonk.fflonk_prove(zkey, wtns, BLINDERS)
     got = proof_from_bytes(raw)
     assert got == want
-    if n_gates < 200:
+    if verify:
         assert fflonk.fflonk_verify(fflonk.fflonk_vk(zkey), public, got)
 
 

@@ -3,6 +3,7 @@ per-element functions the CUDA kernels call (plonk.cuh), compiled with g++ behin
 (tests/host/host_plonk.cpp; NTT / MSM borrowed from the oracle) and compared with oracle/plonk.py proof for proof."""
 import ctypes
 import os
+import re
 import subprocess
 
 import numpy as np
@@ -10,6 +11,8 @@ import pytest
 
 from oracle import oracle as orc
 from oracle import plonk
+
+from tests import r1cs_shapes as S
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BLINDERS = [0x2000 + 7919 * i for i in range(11)]
@@ -77,20 +80,33 @@ def test_host_flow_synthetic(hostlib, n_gates):
     assert plonk.plonk_verify(plonk.plonk_vk(zkey), public, got)
 
 
-@pytest.mark.parametrize("n_gates,n_pub,with_additions", [(29, 3, True), (60, 5, False), (16, 1, False), (8, 2, False)])
+@pytest.mark.parametrize("n_gates,n_pub,with_additions", [(29, 3, True), (60, 5, False), (16, 1, False), (8, 2, False)]
+                         + [pytest.param(label, None, None, id=label) for label in S.PLONK_CASES])
 def test_host_flow_shapes(hostlib, n_gates, n_pub, with_additions):
     """Several public inputs (PI(X) sums several Lagrange polynomials), no additions at all, a gate count equal to the
-    domain size, and the minimum domain (8)."""
-    gates, adds, n_vars, n_pub, wit = plonk.chain_gates(n_gates, n_pub=n_pub, with_additions=with_additions)
-    zkey = plonk.plonk_setup_synth(gates, adds, n_vars, n_pub, tau=31337 + n_gates)
-    wtns = plonk.wtns_bytes(wit)
-    rc, err, raw = host_prove(hostlib, zkey, wtns, BLINDERS)
+    domain size, and the minimum domain (8).  A label instead of a gate count takes the key plonk_setup builds from a
+    circuit of tests/r1cs_shapes.py; where the reference rejects it, the flow gives the same text."""
+    if isinstance(n_gates, str):
+        circ = S.case(n_gates)
+        zkey, wtns, ci, verify = S.plonk_zkey(n_gates), circ.wtns(), orc.CURVES[circ.curve], S.PLONK_CASES[n_gates][3]
+        n_pub = circ.n_public
+    else:
+        gates, adds, n_vars, n_pub, wit = plonk.chain_gates(n_gates, n_pub=n_pub, with_additions=with_additions)
+        zkey = plonk.plonk_setup_synth(gates, adds, n_vars, n_pub, tau=31337 + n_gates)
+        wtns, ci, verify = plonk.wtns_bytes(wit), orc.CURVES[orc.BN254], True
+    rc, err, raw = host_prove(hostlib, zkey, wtns, BLINDERS, ci)
+    if n_gates in S.PLONK_ERRORS:
+        assert rc != 0 and err == S.PLONK_ERRORS[n_gates]
+        with pytest.raises(ValueError, match=re.escape(err)):
+            plonk.plonk_prove(zkey, wtns, BLINDERS)
+        return
     assert rc == 0, err
     want, public = plonk.plonk_prove(zkey, wtns, BLINDERS)
     assert len(public) == n_pub
-    got = proof_from_bytes(raw)
+    got = proof_from_bytes(raw, ci)
     assert got == want
-    assert plonk.plonk_verify(plonk.plonk_vk(zkey), public, got)
+    if verify:
+        assert plonk.plonk_verify(plonk.plonk_vk(zkey), public, got)
 
 
 def test_host_flow_reference_circuit2(hostlib, golden, reference_plonk_key):

@@ -7,6 +7,8 @@ import pytest
 from oracle import fflonk
 from oracle import oracle as orc
 
+from tests import r1cs_shapes as S
+
 BLINDERS = [0x4000 + 1299709 * i for i in range(9)]
 
 
@@ -68,3 +70,39 @@ def test_fflonk_setup_reproduces_reference_zkey_byte_for_byte(golden, ref_case):
     g = golden("plonk_setup_cases.npz")
     ptau = orc.write_binfile("ptau", 1, [(1, bytes(g["ptau_header"])), (2, bytes(g["ff256_ptau2"])), (3, bytes(g["ptau3"])), (12, b"")])
     assert fflonk.fflonk_setup(bytes(g["ff256_r1cs"]), ptau) == ref_case["zkey"]
+
+
+# ----------------------------------------------------------------------------- keys from tests/r1cs_shapes.py circuits
+SHAPES_STRUCTURED = [label for label, c in S.PLONK_CASES.items()
+                     if c[3] and c[1] == orc.BN254 and label not in S.FFLONK_ERRORS]
+
+
+@pytest.mark.parametrize("label", SHAPES_STRUCTURED)
+def test_shape_keys_prove_and_verify(label):
+    """fflonk_setup over a ptau with known tau, for circuits shaped like circom output, including nPublic = 0 (fflonk
+    reads the whole Lagrange section, fflonk_prove.js, so it proves such keys)."""
+    circ = S.case(label)
+    zkey = S.fflonk_zkey(label)
+    proof, public = fflonk.fflonk_prove(zkey, circ.wtns(), BLINDERS)
+    assert public == [str(x) for x in circ.public()]
+    vk = fflonk.fflonk_vk(zkey)
+    assert fflonk.fflonk_verify(vk, public, proof), label
+    bad = copy.deepcopy(proof)
+    bad["evaluations"]["qc"] = str((int(proof["evaluations"]["qc"]) + 1) % orc.P_BN_R)
+    assert not fflonk.fflonk_verify(vk, public, bad), label
+
+
+@pytest.mark.parametrize("k,extra,n_gates,domain", [(8, -2, 254, 256), (8, -1, 255, 512), (8, 0, 256, 512), (8, 1, 257, 512),
+                                                    (12, 0, 4096, 8192), (12, 1, 4097, 8192)])
+def test_gates_cases_land_on_their_domain(k, extra, n_gates, domain):
+    """fflonk keeps the last two rows for blinding: 2^k - 2 gates fill the domain, 2^k - 1 double it."""
+    zk = fflonk.read_fflonk_zkey(S.fflonk_zkey(f"gates{k}{extra:+d}"))
+    assert (zk["nConstraints"], zk["domainSize"], zk["nAdditions"], zk["nPublic"]) == (n_gates, domain, 0, 2)
+
+
+def test_repeated_signal_gives_a_key_that_does_not_divide():
+    """r1cs_constraint_processor.js keys a linear combination by signal as plonk_setup.js does: a repeated signal keeps
+    only its last entry, and the key no longer encodes the circuit."""
+    assert S.FFLONK_ERRORS["coeffs"] == "Polynomial is not divisible"
+    with pytest.raises(ValueError, match="^Polynomial is not divisible$"):
+        fflonk.fflonk_prove(S.fflonk_zkey("coeffs"), S.case("coeffs").wtns(), BLINDERS)

@@ -6,6 +6,8 @@ import pytest
 from oracle import oracle as orc
 from oracle import plonk
 
+from tests import r1cs_shapes as S
+
 BLINDERS = [0x1000 + 977 * i for i in range(11)]
 
 
@@ -112,3 +114,48 @@ def test_plonk_setup_reproduces_reference_zkeys_byte_for_byte(golden, reference_
     bad = dict(proof)
     bad["eval_s1"] = str((int(proof["eval_s1"]) + 1) % orc.P_BN_R)
     assert not plonk.plonk_verify(plonk.plonk_vk(zkey), public, bad)
+
+
+# ----------------------------------------------------------------------------- keys from tests/r1cs_shapes.py circuits
+SHAPES_STRUCTURED = [label for label, c in S.PLONK_CASES.items() if c[3] and label not in S.PLONK_ERRORS]
+
+
+@pytest.mark.parametrize("label", SHAPES_STRUCTURED)
+def test_shape_keys_prove_and_verify(label):
+    """plonk_setup over a ptau with known tau, for circuits shaped like circom output: the proof verifies, and its public
+    signals are the circuit's."""
+    circ = S.case(label)
+    zkey = S.plonk_zkey(label)
+    proof, public = plonk.plonk_prove(zkey, circ.wtns(), BLINDERS)
+    assert public == [str(x) for x in circ.public()]
+    vk = plonk.plonk_vk(zkey)
+    assert plonk.plonk_verify(vk, public, proof), label
+    bad = dict(proof)
+    bad["eval_b"] = str((int(proof["eval_b"]) + 1) % circ.r)
+    assert not plonk.plonk_verify(vk, public, bad), label
+
+
+@pytest.mark.parametrize("k,extra,n_gates,domain", [(8, 0, 256, 256), (8, 1, 257, 512), (8, -2, 254, 256), (8, -1, 255, 256),
+                                                    (12, 0, 4096, 4096), (12, 1, 4097, 8192)])
+def test_gates_cases_land_on_their_domain(k, extra, n_gates, domain):
+    zk = plonk.read_plonk_zkey(S.plonk_zkey(f"gates{k}{extra:+d}"))
+    assert (zk["nConstraints"], zk["domainSize"], zk["nAdditions"], zk["nPublic"]) == (n_gates, domain, 0, 2)
+
+
+def test_repeated_signal_gives_a_key_that_does_not_divide():
+    """plonk_setup keys a linear combination by signal, so a signal twice in one keeps only its last entry (plonk_setup.js:
+    147-149): the gates no longer encode the constraint, and T is not divisible by Z_H, as in the reference."""
+    assert S.PLONK_ERRORS["coeffs"] == "Polynomial is not divisible"
+    with pytest.raises(ValueError, match="^Polynomial is not divisible$"):
+        plonk.plonk_prove(S.plonk_zkey("coeffs"), S.case("coeffs").wtns(), BLINDERS)
+
+
+@pytest.mark.parametrize("label", ["public0", "tiny1"])
+def test_key_without_public_signals_is_refused_with_the_reference_text(label):
+    """With nPublic = 0 the reference reads no Lagrange polynomial (plonk_prove.js:503-509), and round 3's first read of
+    L1 throws (:613-617, evaluations.js:39-44)."""
+    circ = S.case(label)
+    zkey = S.plonk_zkey(label)
+    assert plonk.read_plonk_zkey(zkey)["nPublic"] == 0
+    with pytest.raises(ValueError, match=r"^Evaluations\.getEvaluation\(\) out of bounds$"):
+        plonk.plonk_prove(zkey, circ.wtns(), BLINDERS)
