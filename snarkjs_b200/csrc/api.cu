@@ -77,9 +77,10 @@ struct Groth16Key {
     uint64_t* d_rowptr = nullptr; uint32_t* d_sig = nullptr; void* d_coef = nullptr; uint64_t nCoef = 0;
     // device work buffers
     bool witness_resident = false;   // set by the first upload: sb_groth16_prove_resident refuses to run before it
-    void *dW = nullptr, *dA_T = nullptr, *dB_T = nullptr, *dC_T = nullptr, *dTmp = nullptr, *dTmp2 = nullptr, *dTmp3 = nullptr, *dWsum = nullptr;
+    void *dW = nullptr, *dWsum = nullptr;
     size_t wsum_bytes = 0;           // size of dWsum (groth16_wsum_room grows it)
-    // sb_groth16_prove_batch, grown to the largest sub-batch: K' witnesses, the 3K' transforms and their scratch
+    // sb_groth16_prove_batch's K witnesses, and the transforms of K proofs with their scratch (3Kn elements each: loaded
+    // for one proof, grown by the batch to its largest sub-batch)
     DevBuf batchW, batchX, batchY;
 };
 
@@ -399,9 +400,35 @@ void tick(sb_ctx* c, int i) { cudaEventRecord(c->ev[i], c->stream); }
 float elapsed(sb_ctx* c, int a, int b) { float ms = 0; cudaEventElapsedTime(&ms, c->ev[a], c->ev[b]); return ms; }
 
 // ------------------------------------------------------------------------------------------------------------
-// MSM over device-resident bases/scalars: sort once, one bucket pipeline, host recombination.
-// acc (host XYZZ bytes) += result
+// MSMs over device-resident bases/scalars: sort once, one bucket pipeline, host recombination.
 // ------------------------------------------------------------------------------------------------------------
+// rows MSMs of n scalars each over one base set (row q's scalars at d_sc + q * n * sb, on the device), sorted and reduced
+// together: one sort with MsmGeom::K = rows, one bucket pipeline, one download of the window sums, and each row recombined
+// on its own into out (rows x XYZZ, accumulated into).  g is the set's geometry (table mode: the table's, with first and W
+// set); rows must not exceed msm_batch_limit, and n one MSM chunk.
+int msm_rows_dev(sb_ctx* c, const GroupOps& G, const void* d_bases, const MsmGeom& g, const uint8_t* d_sc, uint32_t sb, uint64_t n,
+                 uint32_t rows, uint8_t* out) {
+    const size_t wrow = (size_t)msm_wsum_parts(g) * g.windows_per_proof() * G.xyzz_bytes;   // window-sum bytes of one row
+    MsmGeom gK = g; gK.K = rows;
+    void* d_wsum = c->io[3].get(rows * wrow);
+    if (!d_wsum) return fail(c, SB_ERR_NOMEM, "out of device memory");
+    MsmSorted srt;
+    int rc = msm_sort_entries(d_sc, sb, n, gK, c->sort_scratch, c->stream, &srt, &c->stats);
+    if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
+    c->stats.cur_tag = (&G == &c->g1) ? SB_G1 : SB_G2;
+    rc = G.buckets(d_bases, srt, c->bucket_scratch, c->stream, d_wsum, &c->stats, nullptr, nullptr);
+    if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_buckets");
+    std::vector<uint8_t> ws(rows * wrow);
+    uint64_t entries = 0;
+    CU(c, cudaMemcpyAsync(ws.data(), d_wsum, ws.size(), cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaMemcpyAsync(&entries, srt.counts, 8, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+    c->stat[(&G == &c->g1) ? 4 : 5] += (double)entries;
+    for (uint32_t q = 0; q < rows; q++) G.combine(ws.data() + q * wrow, g, out + (size_t)q * G.xyzz_bytes);
+    return 0;
+}
+
+// One MSM of any length, chunk by chunk: acc (host XYZZ bytes) += result
 int msm_dev_accumulate(sb_ctx* c, const GroupOps& G, const void* d_bases, const uint8_t* d_scalars, uint32_t sbytes, uint64_t n,
                        uint8_t* acc_xyzz, const MsmGeom* gp = nullptr, uint64_t first = 0) {
     const uint64_t MAXC = 1ull << (g_msm_chunk_log > 0 ? g_msm_chunk_log : 23);   // points per MSM chunk
@@ -411,21 +438,9 @@ int msm_dev_accumulate(sb_ctx* c, const GroupOps& G, const void* d_bases, const 
         if (gp) {   // registered set with precomputed window multiples: d_bases is the table
             g = *gp; g.first = first + off; g.W = (int)((8 * sbytes + 1 + g.c - 1) / g.c);
         }
-        MsmSorted s;
-        int rc = msm_sort_entries(d_scalars + off * sbytes, sbytes, cn, g, c->sort_scratch, c->stream, &s, &c->stats);
-        if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
-        void* d_wsum = c->io[3].get((size_t)g.wsum_points() * G.xyzz_bytes);
-        if (!d_wsum) return fail(c, SB_ERR_NOMEM, "out of device memory");
-        c->stats.cur_tag = (&G == &c->g1) ? SB_G1 : SB_G2;
-        rc = G.buckets(gp ? d_bases : (const void*)((const uint8_t*)d_bases + off * G.aff_bytes), s, c->bucket_scratch, c->stream, d_wsum, &c->stats, nullptr, nullptr);
-        if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_buckets");
-        std::vector<uint8_t> ws((size_t)g.wsum_points() * G.xyzz_bytes);
-        uint64_t entries = 0;
-        CU(c, cudaMemcpyAsync(ws.data(), d_wsum, ws.size(), cudaMemcpyDeviceToHost, c->stream));
-        CU(c, cudaMemcpyAsync(&entries, s.counts, 8, cudaMemcpyDeviceToHost, c->stream));
-        CU(c, cudaStreamSynchronize(c->stream));
-        c->stat[(&G == &c->g1) ? 4 : 5] += (double)entries;
-        G.combine(ws.data(), g, acc_xyzz);
+        int rc = msm_rows_dev(c, G, gp ? d_bases : (const void*)((const uint8_t*)d_bases + off * G.aff_bytes), g, d_scalars + off * sbytes,
+                              sbytes, cn, 1, acc_xyzz);
+        if (rc) return rc;
     }
     return 0;
 }
@@ -464,7 +479,7 @@ int msm_host_inputs(sb_ctx* c, int group, const uint8_t* bases, const void* d_ba
 }
 
 void free_key(Groth16Key* k) {
-    for (void* p : {k->tA, k->tB1, k->tB2, k->tC, k->tH, k->dA, k->dB1, k->dB2, k->dC, k->dH, (void*)k->d_rowptr, (void*)k->d_sig, k->d_coef, k->dW, k->dA_T, k->dB_T, k->dC_T, k->dTmp, k->dTmp2, k->dTmp3, k->dWsum})
+    for (void* p : {k->tA, k->tB1, k->tB2, k->tC, k->tH, k->dA, k->dB1, k->dB2, k->dC, k->dH, (void*)k->d_rowptr, (void*)k->d_sig, k->d_coef, k->dW, k->dWsum})
         if (p) cudaFree(p);
     k->batchW.release(); k->batchX.release(); k->batchY.release();
     delete k;
@@ -642,36 +657,6 @@ static uint32_t batch_size(sb_ctx* c, uint32_t count, uint64_t key_limit, size_t
     return (uint32_t)std::max<uint64_t>(kb, 1);
 }
 
-// rows MSMs of n scalars each over one base set (row q's scalars at d_sc + q * n * sb, on the device), sorted and reduced
-// together: one sort with MsmGeom::K = rows, one bucket pipeline, one download of the window sums, and each row recombined
-// on its own into out (rows x XYZZ).  g is the set's geometry (table mode: the table's, with first and W set); rows must
-// not exceed msm_batch_limit, and n one MSM chunk.
-static int msm_rows_dev(sb_ctx* c, const GroupOps& G, const void* d_bases, const MsmGeom& g, const uint8_t* d_sc, uint32_t sb, uint64_t n,
-                        uint32_t rows, uint8_t* out) {
-    const size_t wrow = (size_t)msm_wsum_parts(g) * g.windows_per_proof() * G.xyzz_bytes;   // window-sum bytes of one row
-    MsmGeom gK = g; gK.K = rows;
-    void* d_wsum = c->io[3].get(rows * wrow);
-    if (!d_wsum) return fail(c, SB_ERR_NOMEM, "out of device memory");
-    MsmSorted srt;
-    int rc = msm_sort_entries(d_sc, sb, n, gK, c->sort_scratch, c->stream, &srt, &c->stats);
-    if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
-    c->stats.cur_tag = (&G == &c->g1) ? SB_G1 : SB_G2;
-    rc = G.buckets(d_bases, srt, c->bucket_scratch, c->stream, d_wsum, &c->stats, nullptr, nullptr);
-    if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_buckets");
-    std::vector<uint8_t> ws(rows * wrow);
-    uint64_t entries = 0;
-    CU(c, cudaMemcpyAsync(ws.data(), d_wsum, ws.size(), cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaMemcpyAsync(&entries, srt.counts, 8, cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
-    c->stat[(&G == &c->g1) ? 4 : 5] += (double)entries;
-    for (uint32_t q = 0; q < rows; q++) {
-        uint8_t* acc = out + (size_t)q * G.xyzz_bytes;
-        memset(acc, 0, G.xyzz_bytes);
-        G.combine(ws.data() + q * wrow, g, acc);
-    }
-    return 0;
-}
-
 // count MSMs over the same registered bases: the rows are sorted and reduced together in sub-batches (MsmGeom::K), each row
 // recombined on its own.  Rows longer than an MSM chunk (2^23 points) go one by one through sb_msm_registered's path.
 int sb_msm_registered_batch(sb_ctx* c, uint64_t h, uint64_t first, const uint8_t* scalars, uint32_t sb, uint64_t n, uint32_t count, uint8_t* out) { SB_LOCK(c);
@@ -705,6 +690,7 @@ int sb_msm_registered_batch(sb_ctx* c, uint64_t h, uint64_t first, const uint8_t
     prof_begin(c);
     for (uint32_t r0 = 0; r0 < count; r0 += KB) {
         const uint32_t kb = std::min(KB, count - r0);
+        std::fill(sums.begin(), sums.end(), 0);
         uint8_t* d_sc = (uint8_t*)c->io[1].get((size_t)kb * n * sb);
         if (!d_sc) return fail(c, SB_ERR_NOMEM, "out of device memory");
         CU(c, h2d(c, d_sc, scalars + (size_t)r0 * n * sb, (size_t)kb * n * sb));
@@ -1014,7 +1000,7 @@ static int groth16_load_impl(sb_ctx* c, const uint8_t* zkey, uint64_t zlen, int 
     up((void**)&k->d_sig, z.sig.data(), z.sig.size() * 4);
     up(&k->d_coef, z.coef.data(), z.coef.size());
     alloc(&k->dW, (nv + 64) * 32);   // + room for the padded slices of the distributed witness all-gather
-    for (void** d : {&k->dA_T, &k->dB_T, &k->dC_T, &k->dTmp, &k->dTmp2, &k->dTmp3}) alloc(d, n * 32);
+    if (e == cudaSuccess && (!k->batchX.get(3 * n * 32) || !k->batchY.get(3 * n * 32))) e = cudaErrorMemoryAllocation;
     alloc(&k->dWsum, 8 * 80 * 4 * 96);
     if (e == cudaSuccess) k->wsum_bytes = 8 * 80 * 4 * 96;
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);   // the CSR vectors and the caller's bytes go away on return
@@ -1162,16 +1148,202 @@ static int groth16_wsum_room(sb_ctx* c, Groth16Key* k, size_t dev_bytes, size_t 
     return 0;
 }
 
+// QAP rows -> iNTT -> coset NTT -> [exchange] -> joinABC of K proofs (witness q at dW + q * nVars elements) on stream st, in
+// the key's transform buffers batchX / batchY (3Kn elements each: A of every proof, then B, then C).  *hsc = where the H
+// scalars went (proof q's at + q * n elements); the ones of [hlo, hlo + hcnt) are computed, K > 1 only with the full range.
+// dist: the three chains run on the ranks sb_dist_chain_owner names and send their coset evaluations to every other rank's
+// H range (NCCL send/recv); every rank then joins its own H range.
+static int groth16_qap_ntt(sb_ctx* c, Groth16Key* k, const void* dW, uint32_t K, uint64_t hlo, uint64_t hcnt, bool dist,
+                           cudaStream_t st, uint8_t** hsc) {
+    const int cv = c->curve;
+    const uint64_t n = k->domainSize, nv = k->nVars;
+    const size_t tn = (size_t)K * n * 32;   // bytes of one of A, B, C over the K proofs
+    uint8_t* X = (uint8_t*)k->batchX.get(3 * tn);
+    uint8_t* Y = (uint8_t*)k->batchY.get(3 * tn);
+    if (!X || !Y) return fail(c, SB_ERR_NOMEM, "out of device memory (Groth16 transform buffers)");
+    const bool xchg = dist && c->world > 1;
+    // Every pass moves the data to the other buffer, so where the coset evaluations end up follows from the pass count:
+    // known on ranks that run no chain too, which receive into it.
+    const int np = fr_ntt_passes(k->power);
+    auto after_ntt = [&](uint8_t* in) { return (np & 1) ? (in == X ? Y : X) : in; };
+    uint8_t* const ev = after_ntt(after_ntt(X));
+    int my[3], m = 0;
+    for (int j = 0; j < 3; j++) if (!xchg || sb_dist_chain_owner(j, c->world) == c->rank) my[m++] = j;
+    int rc;
+    if (m) {
+        // buildABC1 (:147-187)
+        { ProfScope pq(&c->stats, PROF_QAP, st);
+          rc = fr_qap_rows(cv, k->d_rowptr, k->d_sig, k->d_coef, dW, nv, X, X + tn, X + 2 * tn, n, K, st); c->launches++;
+          pq.end(); }
+        if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_qap_rows");
+        // :64-76  ifft -> batchApplyKey(1, inc) -> fft, with 1/n of the inverse folded into the coset table
+        const uint8_t* inc = (k->power == c->fr_s) ? c->shift.data() : c->roots[k->power + 1].data();
+        uint8_t ninv[32];
+        if (cv == SB_BN254) ninv_bytes<BnFr>(k->power, ninv); else ninv_bytes<BlsFr>(k->power, ninv);
+        FrPre pre; rc = get_pre(c, n, ninv, inc, &pre); if (rc) return rc;
+        FrNttTables tbi, tbf;
+        rc = get_ntt_tab(c, k->power, true, &tbi); if (rc) return rc;
+        rc = get_ntt_tab(c, k->power, false, &tbf); if (rc) return rc;
+        // the transforms run as one batch per pass (grids fill whole waves): up to four by pointer (one proof's chains, or
+        // the ones this rank owns, which need not be adjacent), more as one strided batch of all 3K
+        int side = 0, side2 = 0, launches = 0;
+        bool landed;
+        ProfScope pn(&c->stats, PROF_NTT, st);
+        if (m * K <= 4) {
+            void* a[4]; void* b[4]; int t = 0;
+            for (int i = 0; i < m; i++)
+                for (uint32_t q = 0; q < K; q++, t++) { const size_t o = my[i] * tn + q * n * 32; a[t] = X + o; b[t] = Y + o; }
+            rc = fr_ntt_batch(cv, a, b, t, k->power, &tbi, nullptr, nullptr, st, &side, &launches);      // unscaled inverse
+            if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_ntt_batch");
+            void** src = side ? b : a; void** dst = side ? a : b;
+            rc = fr_ntt_batch(cv, src, dst, t, k->power, &tbf, &pre, nullptr, st, &side2, &launches);     // coset NTT, 1/n folded in
+            if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_ntt_batch");
+            landed = (side2 ? dst : src)[0] == ev + my[0] * tn;
+        } else {
+            rc = fr_ntt_strided(cv, X, Y, 3 * (int)K, k->power, &tbi, nullptr, nullptr, st, &side, &launches);
+            if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_ntt_strided");
+            uint8_t* src = side ? Y : X; uint8_t* dst = side ? X : Y;
+            rc = fr_ntt_strided(cv, src, dst, 3 * (int)K, k->power, &tbf, &pre, nullptr, st, &side2, &launches);
+            if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_ntt_strided");
+            landed = (side2 ? dst : src) == ev;
+        }
+        pn.end();
+        c->launches += launches;
+        if (!landed) return fail(c, SB_ERR_CUDA, "internal: NTT result buffer mismatch");
+    }
+    if (xchg) {   // coset evaluations of chain j: owner -> every other rank's H range
+        NcclApi* nc = nccl_api(nullptr);
+        NC(c, nc, nc->GroupStart());
+        for (int j = 0; j < 3; j++) {
+            const int o = sb_dist_chain_owner(j, c->world);
+            uint8_t* evj = ev + j * tn;
+            if (o == c->rank) {
+                for (int q = 0; q < c->world; q++) {
+                    if (q == c->rank) continue;
+                    uint64_t qlo, qcnt; sb_shard_range(n, q, c->world, &qlo, &qcnt);
+                    if (qcnt) NC(c, nc, nc->Send(evj + qlo * 32, qcnt * 32, ncclUint8, q, c->comm, st));
+                }
+            } else if (hcnt) NC(c, nc, nc->Recv(evj + hlo * 32, hcnt * 32, ncclUint8, o, c->comm, st));
+        }
+        NC(c, nc, nc->GroupEnd());
+    }
+    // joinABC (:320-374) -> plain scalars for the H MSM, into the other buffer (free once the transforms are done)
+    uint8_t* const h = ev == X ? Y : X;
+    if (hcnt) {
+        ProfScope pj(&c->stats, PROF_JOIN, st);
+        rc = fr_join_abc(cv, ev + hlo * 32, ev + tn + hlo * 32, ev + 2 * tn + hlo * 32, h + hlo * 32, K * hcnt, st); c->launches++;
+        pj.end();
+        if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_join_abc");
+    }
+    *hsc = h;
+    return 0;
+}
+
+// One of the five MSMs of a sub-batch: its group, one proof's geometry (what combine takes), its window sums in the pinned
+// area (len bytes at off, proof q's at off + q * per) and the offset of its partial in a proof's A | B1 | C | H | B2.
+struct Groth16Job { const GroupOps* G; MsmGeom g; size_t off, len, per, part; };
+struct Groth16Jobs {
+    Groth16Job job[5];        // A, B1, B2, C, H: the order they are issued and land in; H's region ends the area
+    const uint64_t* counts;   // pinned: the sorted entries of the witness and of the H digits
+    // sb_last_stat 4 and 5, once every job has landed
+    void tally(sb_ctx* c) const { c->stat[4] += 3.0 * (double)counts[0] + (double)counts[1]; c->stat[5] += (double)counts[0]; }
+};
+
+// The device work of K proofs (witness q at dW + q * nVars elements) over the witness points [wlo, wlo + wcnt) and the H
+// points [hlo, hlo + hcnt), each at most one MSM chunk; K > 1 only with the full ranges.  The witness is sorted once (A,
+// B1, B2 and C all multiply it, :84-97); the five bucket pipelines run on their own streams so that the latency-bound
+// tails (fold cascade, bucket reduction) of one MSM hide under the throughput-bound accumulation of the next; the H
+// scalars (QAP/NTT chain) are produced concurrently.  g_serial_prove serialises everything on one stream (profiling).
+//   main stream  : sort(witness), acc A, acc B1, acc B2, acc C, [wait for the NTT chain], acc H
+//   aux[5] (hi)  : QAP -> iNTT -> coset NTT -> [exchange] -> joinABC -> sort(H scalars)
+//   aux[0..4](hi): the tail of MSM i (fold, reduce, window sum) and its D2H into the pinned area, then pev[2 + i]
+// Returns with the work queued and the main stream waiting for all of it; job i's window sums are on the host once
+// pev[2 + i] has fired.
+static int groth16_issue(sb_ctx* c, Groth16Key* k, const void* dW, uint32_t K, uint64_t wlo, uint64_t wcnt, uint64_t hlo, uint64_t hcnt,
+                         bool dist, Groth16Jobs* out) {
+    const GroupOps& G1 = c->g1; const GroupOps& G2 = c->g2;
+    const uint32_t x1 = G1.xyzz_bytes, x2 = G2.xyzz_bytes;
+    const bool serial = g_serial_prove != 0;
+    cudaStream_t s0 = c->stream, sN = serial ? s0 : c->aux[5];
+    // a key loaded with sb_groth16_load_sharded only holds its own ranges: local indexing
+    const bool local = k->n_shards > 1;
+    const uint64_t wb = local ? 0 : wlo, hb = local ? 0 : hlo;   // base-set index of the first point
+    const bool pre = k->tA != nullptr;
+    MsmGeom gw = msm_geometry(wcnt, 32, c->fr_bits), gh = msm_geometry(hcnt, 32, c->fr_bits);
+    if (pre) { gw = k->gpW; gw.first = wb; gh = k->gpH; gh.first = hb; }
+    MsmGeom gwK = gw, ghK = gh; gwK.K = K; ghK.K = K;
+    const size_t w1 = (size_t)gwK.wsum_points() * x1, w2 = (size_t)gwK.wsum_points() * x2, wh = (size_t)ghK.wsum_points() * x1;
+    const size_t wtot = 3 * w1 + w2 + wh;
+    int rc = groth16_wsum_room(c, k, wtot, wtot + 64);
+    if (rc) return rc;
+    uint8_t* dws = (uint8_t*)k->dWsum; uint8_t* hws = c->pinned;
+    uint64_t* hcounts = (uint64_t*)(c->pinned + wtot);
+    CU(c, cudaEventRecord(c->pev[0], s0));                       // witnesses resident
+    if (sN != s0) CU(c, cudaStreamWaitEvent(sN, c->pev[0], 0));
+    // NTT chain + sort of the H scalars on the side stream
+    uint8_t* hsc;
+    rc = groth16_qap_ntt(c, k, dW, K, hlo, hcnt, dist, sN, &hsc);
+    if (rc) return rc;
+    MsmSorted sh;
+    rc = msm_sort_entries(hsc + hlo * 32, 32, hcnt, ghK, c->sort_scratch2, sN, &sh, &c->stats);
+    if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
+    CU(c, cudaEventRecord(c->pev[1], sN));
+    // witness MSMs on the main stream
+    MsmSorted sw;
+    rc = msm_sort_entries((const uint8_t*)dW + wlo * 32, 32, wcnt, gwK, c->sort_scratch, s0, &sw, &c->stats);
+    if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
+    tick(c, 2);
+    // A and B1 first (a single proof folds s*A + r*B1 on the host as they land), then the long G2 MSM, C, and H last
+    const size_t pw = (size_t)msm_wsum_parts(gw) * gw.windows_per_proof(), ph = (size_t)msm_wsum_parts(gh) * gh.windows_per_proof();
+    *out = Groth16Jobs{{{&G1, gw, 0, w1, pw * x1, 0}, {&G1, gw, w1, w1, pw * x1, x1}, {&G2, gw, 3 * w1, w2, pw * x2, 4 * x1},
+                        {&G1, gw, 2 * w1, w1, pw * x1, 2 * x1}, {&G1, gh, 3 * w1 + w2, wh, ph * x1, 3 * x1}}, hcounts};
+    const void* bases[5] = {pre ? k->tA : (const void*)((const uint8_t*)k->dA + wb * G1.aff_bytes),
+                            pre ? k->tB1 : (const void*)((const uint8_t*)k->dB1 + wb * G1.aff_bytes),
+                            pre ? k->tB2 : (const void*)((const uint8_t*)k->dB2 + wb * G2.aff_bytes),
+                            pre ? k->tC : (const void*)((const uint8_t*)k->dC + wb * G1.aff_bytes),
+                            pre ? k->tH : (const void*)((const uint8_t*)k->dH + hb * G1.aff_bytes)};
+    for (int i = 0; i < 5; i++) {
+        const Groth16Job& j = out->job[i];
+        cudaStream_t st = serial ? s0 : c->aux[i];
+        if (i == 4 && sN != s0) CU(c, cudaStreamWaitEvent(s0, c->pev[1], 0));   // H needs the NTT chain
+        c->stats.cur_tag = j.G == &G1 ? SB_G1 : SB_G2;
+        rc = j.G->buckets(bases[i], i == 4 ? sh : sw, c->bscr[i], s0, dws + j.off, &c->stats, st, c->pev[8 + i]);
+        if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_buckets");
+        CU(c, cudaMemcpyAsync(hws + j.off, dws + j.off, j.len, cudaMemcpyDeviceToHost, st));
+        if (i == 0) CU(c, cudaMemcpyAsync(&hcounts[0], sw.counts, 8, cudaMemcpyDeviceToHost, st));
+        if (i == 4) CU(c, cudaMemcpyAsync(&hcounts[1], sh.counts, 8, cudaMemcpyDeviceToHost, st));
+        CU(c, cudaEventRecord(c->pev[2 + i], st));
+    }
+    tick(c, 3);
+    // join the side streams back into the main stream
+    if (!serial) { for (int i = 0; i < 5; i++) CU(c, cudaStreamWaitEvent(s0, c->pev[2 + i], 0)); CU(c, cudaStreamWaitEvent(s0, c->pev[1], 0)); }
+    return 0;
+}
+
+// C' = C + H + s*A + r*B1 into the C slot of one proof's partials (A | B1 | C | H | B2): the part of the split assembly
+// (groth16_fixed_parts) that depends on the MSMs.  sA = s*A and rB1 = r*B1, which a single proof computes as A and B1 land.
+static void groth16_fold(const GroupOps& G1, uint8_t* partials, const uint8_t* sA, const uint8_t* rB1) {
+    uint8_t* C = partials + 2 * G1.xyzz_bytes;
+    G1.add(C, partials + 3 * G1.xyzz_bytes); G1.add(C, sA); G1.add(C, rB1);
+}
+static void groth16_fold_scalars(const GroupOps& G1, uint8_t* partials, const ProofScalars& ps) {
+    std::vector<uint8_t> sA(G1.xyzz_bytes), rB1(G1.xyzz_bytes);
+    G1.times(partials, ps.sp, 32, sA.data());                      // s * A   (src/groth16_prove.js:117: pi_c += s*pi_a)
+    G1.times(partials + G1.xyzz_bytes, ps.rp, 32, rB1.data());     // r * B1  (:118)
+    groth16_fold(G1, partials, sA.data(), rB1.data());
+}
+
 // device part of the prover: returns the five MSM partials (A, B1, C, H | B2) as host XYZZ bytes.
+// witness is uploaded to the key's resident witness; null proves from the resident one, or from d_witness when given (a
+// witness already on the device: the resident one is left as it is).
 // dist: this context is rank c->rank of c->world (sb_comm_init_rank); the witness is uploaded in slices and all-gathered,
 // the three transform chains run on different ranks and exchange their coset evaluations (NCCL send/recv), every rank
 // then joins and multiplies its own H range.
 static int groth16_device(sb_ctx* c, Groth16Key* k, const uint8_t* witness, uint64_t n_witness, int shard, int n_shards, uint8_t* partials,
-                          const ProofScalars* ps = nullptr, bool dist = false) {
+                          const ProofScalars* ps = nullptr, bool dist = false, const void* d_witness = nullptr) {
     if (witness && n_witness != k->nVars) return fail(c, SB_ERR_ARG, "Invalid witness length. Circuit: " + std::to_string(k->nVars) + ", witness: " + std::to_string(n_witness));
     cudaSetDevice(c->device);
     const uint64_t n = k->domainSize, nv = k->nVars;
-    const int cv = c->curve;
     NcclApi* nc = nullptr;
     if (dist) {
         if (!c->comm) return fail(c, SB_ERR_ARG, "context has no communicator: call sb_comm_init_rank first");
@@ -1179,6 +1351,7 @@ static int groth16_device(sb_ctx* c, Groth16Key* k, const uint8_t* witness, uint
         shard = c->rank; n_shards = c->world;
     }
     const int world = n_shards, rank = shard;
+    const void* dW = d_witness ? d_witness : k->dW;
     int rc;
     tick(c, 0);
     if (witness) {
@@ -1189,161 +1362,44 @@ static int groth16_device(sb_ctx* c, Groth16Key* k, const uint8_t* witness, uint
             NC(c, nc, nc->AllGather((const uint8_t*)k->dW + per * rank * 32, k->dW, per * 32, ncclUint8, c->comm, c->stream));
         } else CU(c, h2d(c, k->dW, witness, nv * 32));
         k->witness_resident = true;
-    } else if (!k->witness_resident) return fail(c, SB_ERR_ARG, "no witness resident for this proving key: call sb_groth16_prove first");
+    } else if (!d_witness && !k->witness_resident) return fail(c, SB_ERR_ARG, "no witness resident for this proving key: call sb_groth16_prove first");
     tick(c, 1);
     prof_begin(c);
     // MSMs (:84-101).  Shard = contiguous point range (SURVEY §8e); shard 0 of 1 = everything.
-    auto range_of = [&](uint64_t total, int sh, uint64_t& lo, uint64_t& cnt) { sb_shard_range(total, sh, n_shards, &lo, &cnt); };
-    uint64_t wlo, wcnt; range_of(nv, rank, wlo, wcnt);
-    uint64_t hlo, hcnt; range_of(n, rank, hlo, hcnt);
-    // chain j (0 = A, 1 = B, 2 = C) runs on rank owner(j); without a communicator every chain runs here
-    auto owner = [&](int j) { return (dist && world > 1) ? sb_dist_chain_owner(j, world) : rank; };
-    void* bufs[3] = {k->dA_T, k->dB_T, k->dC_T}; void* scr[3] = {k->dTmp, k->dTmp2, k->dTmp3};
-    // where the chain results end up depends only on the pass count: known on ranks that run no chain too
-    const int np = fr_ntt_passes(k->power);
-    void* odd[3]; void* tmp;
-    { const bool x_scr = (np & 1) != 0;                          // after the inverse transform the data sits in scr iff np is odd
-      for (int j = 0; j < 3; j++) { void* X = x_scr ? scr[j] : bufs[j]; void* Y = x_scr ? bufs[j] : scr[j]; odd[j] = (np & 1) ? Y : X; }
-      tmp = (odd[0] == bufs[0]) ? scr[0] : bufs[0]; }
-    auto run_qap_ntt = [&]() -> int {
-        int my[3], m = 0;
-        for (int j = 0; j < 3; j++) if (owner(j) == rank) my[m++] = j;
-        if (m) {
-            // buildABC1 (:147-187)
-            { ProfScope pq(&c->stats, PROF_QAP, c->stream);
-              rc = fr_qap_rows(cv, k->d_rowptr, k->d_sig, k->d_coef, k->dW, nv, k->dA_T, k->dB_T, k->dC_T, n, 1, c->stream); c->launches++;
-              pq.end(); }
-            if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_qap_rows");
-            // :64-76  ifft -> batchApplyKey(1, inc) -> fft, with 1/n of the inverse folded into the coset table
-            const uint8_t* inc = (k->power == c->fr_s) ? c->shift.data() : c->roots[k->power + 1].data();
-            uint8_t ninv[32];
-            if (cv == SB_BN254) ninv_bytes<BnFr>(k->power, ninv); else ninv_bytes<BlsFr>(k->power, ninv);
-            FrPre pre; rc = get_pre(c, n, ninv, inc, &pre); if (rc) return rc;
-            // this rank's transforms run as one batch per pass (grids fill whole waves)
-            void* a[3]; void* b[3];
-            for (int i = 0; i < m; i++) { a[i] = bufs[my[i]]; b[i] = scr[my[i]]; }
-            FrNttTables tbi, tbf;
-            rc = get_ntt_tab(c, k->power, true, &tbi); if (rc) return rc;
-            rc = get_ntt_tab(c, k->power, false, &tbf); if (rc) return rc;
-            int side = 0, launches = 0;
-            ProfScope pn(&c->stats, PROF_NTT, c->stream);
-            rc = fr_ntt_batch(cv, a, b, m, k->power, &tbi, nullptr, nullptr, c->stream, &side, &launches);      // unscaled inverse
-            if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_ntt_batch");
-            void** src = side ? b : a; void** dst = side ? a : b;
-            int side2 = 0;
-            rc = fr_ntt_batch(cv, src, dst, m, k->power, &tbf, &pre, nullptr, c->stream, &side2, &launches);     // coset NTT, 1/n folded in
-            if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_ntt_batch");
-            pn.end();
-            c->launches += launches;
-            void** res = side2 ? dst : src;
-            for (int i = 0; i < m; i++) if (res[i] != odd[my[i]]) return fail(c, SB_ERR_CUDA, "internal: NTT result buffer mismatch");
-        }
-        if (dist && world > 1) {   // coset evaluations of chain j: owner -> every other rank's H range
-            NC(c, nc, nc->GroupStart());
-            for (int j = 0; j < 3; j++) {
-                const int o = owner(j);
-                if (o == rank) {
-                    for (int q = 0; q < world; q++) {
-                        if (q == rank) continue;
-                        uint64_t qlo, qcnt; range_of(n, q, qlo, qcnt);
-                        if (qcnt) NC(c, nc, nc->Send((const uint8_t*)odd[j] + qlo * 32, qcnt * 32, ncclUint8, q, c->comm, c->stream));
-                    }
-                } else if (hcnt) NC(c, nc, nc->Recv((uint8_t*)odd[j] + hlo * 32, hcnt * 32, ncclUint8, o, c->comm, c->stream));
-            }
-            NC(c, nc, nc->GroupEnd());
-        }
-        // joinABC (:320-374) -> plain scalars for the H MSM, over this rank's H range, into the remaining scratch buffer
-        if (hcnt) {
-            ProfScope pj(&c->stats, PROF_JOIN, c->stream);
-            rc = fr_join_abc(cv, (const uint8_t*)odd[0] + hlo * 32, (const uint8_t*)odd[1] + hlo * 32, (const uint8_t*)odd[2] + hlo * 32,
-                             (uint8_t*)tmp + hlo * 32, hcnt, c->stream); c->launches++;
-            pj.end();
-            if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_join_abc");
-        }
-        return 0;
-    };
+    uint64_t wlo, wcnt; sb_shard_range(nv, rank, n_shards, &wlo, &wcnt);
+    uint64_t hlo, hcnt; sb_shard_range(n, rank, n_shards, &hlo, &hcnt);
     const GroupOps& G1 = c->g1; const GroupOps& G2 = c->g2;
     uint8_t* pA = partials; uint8_t* pB1 = pA + G1.xyzz_bytes; uint8_t* pC = pB1 + G1.xyzz_bytes; uint8_t* pH = pC + G1.xyzz_bytes; uint8_t* pB2 = pH + G1.xyzz_bytes;
     memset(partials, 0, 4 * G1.xyzz_bytes + G2.xyzz_bytes);
     std::vector<uint8_t> sA(G1.xyzz_bytes, 0), rB1(G1.xyzz_bytes, 0);
     const uint64_t MAXC = 1ull << (g_msm_chunk_log > 0 ? g_msm_chunk_log : 23);   // points per MSM chunk
-    // a key loaded with sb_groth16_load_sharded only holds its own ranges: local indexing
     const bool local = k->n_shards > 1;
     if (local && (shard != k->shard || n_shards != k->n_shards)) return fail(c, SB_ERR_ARG, "proving key was loaded for a different shard");
     const uint64_t wb = local ? 0 : wlo, hb = local ? 0 : hlo;   // base-set index of this call's first point
     const bool overlapped = wcnt <= MAXC && hcnt <= MAXC && wcnt > 0 && hcnt > 0 && c->pinned;
     if (dist && world > 1 && !overlapped) return fail(c, SB_ERR_ARG, "distributed proving needs at least one point per rank and shards of at most 2^23 points");
     if (overlapped) {
-        // Overlapped pipeline: the witness is sorted once (A, B1, B2 and C all multiply it, :84-97); the four bucket
-        // pipelines run on their own streams so that the latency-bound tails (fold cascade, bucket reduction) of one
-        // MSM hide under the throughput-bound accumulation of the next; the H scalars (QAP/NTT chain) are produced
-        // concurrently on the main stream.  g_serial_prove serialises everything on one stream (profiling).
-        const bool serial = g_serial_prove != 0;
-        cudaStream_t s0 = c->stream;
-        // schedule: main stream  : H2D, sort(witness), acc B2, acc A, acc B1, acc C, [join NTT chain], acc H
-        //           aux[5] (hi)  : QAP -> iNTT -> coset NTT -> [exchange] -> joinABC -> sort(H scalars)
-        //           aux[0..4](hi): the latency-bound tail of each MSM (fold, reduce, window sum, D2H)
-        cudaStream_t sN = serial ? s0 : c->aux[5];
-        MsmGeom gw = msm_geometry(wcnt, 32, c->fr_bits), gh = msm_geometry(hcnt, 32, c->fr_bits);
-        const bool pre = k->tA != nullptr;
-        if (pre) { gw = k->gpW; gw.first = wb; gh = k->gpH; gh.first = hb; }
-        const size_t w1 = (size_t)gw.wsum_points() * G1.xyzz_bytes, w2 = (size_t)gw.wsum_points() * G2.xyzz_bytes, wh = (size_t)gh.wsum_points() * G1.xyzz_bytes;
-        rc = groth16_wsum_room(c, k, 3 * w1 + w2 + wh, 3 * w1 + w2 + wh + 64);
+        Groth16Jobs t;
+        rc = groth16_issue(c, k, dW, 1, wlo, wcnt, hlo, hcnt, dist, &t);
         if (rc) return rc;
-        uint8_t* dws = (uint8_t*)k->dWsum; uint8_t* hws = c->pinned;
-        uint64_t* hcounts = (uint64_t*)(c->pinned + 3 * w1 + w2 + wh);
-        CU(c, cudaEventRecord(c->pev[0], s0));                       // witness resident
-        if (sN != s0) CU(c, cudaStreamWaitEvent(sN, c->pev[0], 0));
-        // NTT chain + sort of the H scalars on the side stream
-        cudaStream_t saved = c->stream; c->stream = sN;
-        rc = run_qap_ntt();
-        MsmSorted sh;
-        if (!rc) { rc = msm_sort_entries((const uint8_t*)tmp + hlo * 32, 32, hcnt, gh, c->sort_scratch2, sN, &sh, &c->stats); if (rc) rc = cuda_fail(c, (cudaError_t)rc, "msm_sort_entries"); }
-        c->stream = saved;
-        if (rc) return rc;
-        CU(c, cudaEventRecord(c->pev[1], sN));
-        // witness MSMs on the main stream
-        MsmSorted sw;
-        rc = msm_sort_entries((const uint8_t*)k->dW + wlo * 32, 32, wcnt, gw, c->sort_scratch, s0, &sw, &c->stats);
-        if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
-        tick(c, 2);
-        struct Job { const GroupOps* G; const void* bases; size_t off; size_t len; uint8_t* dst; int tag; const MsmSorted* srt; const MsmGeom* g; };
-        // order: A and B1 first (their results feed the host-side s*A + r*B1), then the long G2 MSM, C, and H last
-        Job jobs[5] = {{&G1, pre ? k->tA : (const void*)((const uint8_t*)k->dA + wb * G1.aff_bytes), 0, w1, pA, SB_G1, &sw, &gw},
-                       {&G1, pre ? k->tB1 : (const void*)((const uint8_t*)k->dB1 + wb * G1.aff_bytes), w1, w1, pB1, SB_G1, &sw, &gw},
-                       {&G2, pre ? k->tB2 : (const void*)((const uint8_t*)k->dB2 + wb * G2.aff_bytes), 3 * w1, w2, pB2, SB_G2, &sw, &gw},
-                       {&G1, pre ? k->tC : (const void*)((const uint8_t*)k->dC + wb * G1.aff_bytes), 2 * w1, w1, pC, SB_G1, &sw, &gw},
-                       {&G1, pre ? k->tH : (const void*)((const uint8_t*)k->dH + hb * G1.aff_bytes), 3 * w1 + w2, wh, pH, SB_G1, &sh, &gh}};
-        for (int i = 0; i < 5; i++) {
-            cudaStream_t st = serial ? s0 : c->aux[i];
-            if (i == 4 && sN != s0) CU(c, cudaStreamWaitEvent(s0, c->pev[1], 0));   // H needs the NTT chain
-            c->stats.cur_tag = jobs[i].tag;
-            rc = jobs[i].G->buckets(jobs[i].bases, *jobs[i].srt, c->bscr[i], s0, dws + jobs[i].off, &c->stats, st, c->pev[8 + i]);
-            if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_buckets");
-            CU(c, cudaMemcpyAsync(hws + jobs[i].off, dws + jobs[i].off, jobs[i].len, cudaMemcpyDeviceToHost, st));
-            if (i == 0) CU(c, cudaMemcpyAsync(&hcounts[0], sw.counts, 8, cudaMemcpyDeviceToHost, st));
-            if (i == 4) CU(c, cudaMemcpyAsync(&hcounts[1], sh.counts, 8, cudaMemcpyDeviceToHost, st));
-            CU(c, cudaEventRecord(c->pev[2 + i], st));
-        }
-        tick(c, 3);
         // host recombination as each MSM lands (overlaps with the MSMs still running)
         for (int i = 0; i < 5; i++) {
+            const Groth16Job& j = t.job[i];
             CU(c, cudaEventSynchronize(c->pev[2 + i]));
-            jobs[i].G->combine(hws + jobs[i].off, *jobs[i].g, jobs[i].dst);
+            j.G->combine(c->pinned + j.off, j.g, partials + j.part);
             if (ps && i == 0) G1.times(pA, ps->sp, 32, sA.data());      // s * A   (src/groth16_prove.js:117: pi_c += s*pi_a)
             if (ps && i == 1) G1.times(pB1, ps->rp, 32, rB1.data());    // r * B1  (:118)
         }
-        // join the side streams back into the main stream
-        if (!serial) { for (int i = 0; i < 5; i++) CU(c, cudaStreamWaitEvent(s0, c->pev[2 + i], 0)); CU(c, cudaStreamWaitEvent(s0, c->pev[1], 0)); }
-        c->stat[4] += 3.0 * (double)hcounts[0] + (double)hcounts[1]; c->stat[5] += (double)hcounts[0];
+        t.tally(c);
     } else {
-    rc = run_qap_ntt(); if (rc) return rc;
+    uint8_t* hsc;
+    rc = groth16_qap_ntt(c, k, dW, 1, hlo, hcnt, dist, c->stream, &hsc); if (rc) return rc;
     tick(c, 2);
     for (uint64_t off = 0; off < wcnt; off += MAXC) {
         uint64_t cn = std::min(MAXC, wcnt - off), base = wb + off;
         MsmGeom g = msm_geometry(cn, 32, c->fr_bits);
         MsmSorted s;
-        rc = msm_sort_entries((const uint8_t*)k->dW + (wlo + off) * 32, 32, cn, g, c->sort_scratch, c->stream, &s, &c->stats);
+        rc = msm_sort_entries((const uint8_t*)dW + (wlo + off) * 32, 32, cn, g, c->sort_scratch, c->stream, &s, &c->stats);
         if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
         size_t w1 = (size_t)g.wsum_points() * G1.xyzz_bytes, w2 = (size_t)g.wsum_points() * G2.xyzz_bytes;
         rc = groth16_wsum_room(c, k, 3 * w1 + w2, 0);
@@ -1365,13 +1421,13 @@ static int groth16_device(sb_ctx* c, Groth16Key* k, const uint8_t* witness, uint
     }
     tick(c, 3);
     if (hcnt) {
-        rc = msm_dev_accumulate(c, G1, (const uint8_t*)k->dH + hb * G1.aff_bytes, (const uint8_t*)tmp + hlo * 32, 32, hcnt, pH);
+        rc = msm_dev_accumulate(c, G1, (const uint8_t*)k->dH + hb * G1.aff_bytes, hsc + hlo * 32, 32, hcnt, pH);
         if (rc) return rc;
     }
     if (ps) { G1.times(pA, ps->sp, 32, sA.data()); G1.times(pB1, ps->rp, 32, rB1.data()); }
     }
     if (ps) {   // C' = C + H + s*A + r*B1;  the B1 and H slots are spent
-        G1.add(pC, pH); G1.add(pC, sA.data()); G1.add(pC, rB1.data());
+        groth16_fold(G1, partials, sA.data(), rB1.data());
         memset(pB1, 0, G1.xyzz_bytes); memset(pH, 0, G1.xyzz_bytes);
     }
     tick(c, 4);
@@ -1384,65 +1440,31 @@ static int groth16_device(sb_ctx* c, Groth16Key* k, const uint8_t* witness, uint
 // host part: proof assembly, src/groth16_prove.js:103-132
 
 struct VkPoints { const uint8_t *alpha1, *beta1, *beta2, *delta1, *delta2; };
-static void plain_scalars(int curve, const uint8_t r[32], const uint8_t s[32], uint8_t rp[32], uint8_t sp[32], uint8_t rsp[32], bool negate_rs) {
+static void plain_scalars(int curve, const uint8_t r[32], const uint8_t s[32], uint8_t rp[32], uint8_t sp[32], uint8_t rsp[32]) {
     uint8_t rs[32];
     if (curve == SB_BN254) {
         fr_from_mont_bytes<BnFr>(r, rp); fr_from_mont_bytes<BnFr>(s, sp);
-        Fp<BnFr> a, b; memcpy(&a, r, 32); memcpy(&b, s, 32); a = Fp<BnFr>::mul(a, b); if (negate_rs) a = Fp<BnFr>::neg(a); memcpy(rs, &a, 32);
+        Fp<BnFr> a, b; memcpy(&a, r, 32); memcpy(&b, s, 32); a = Fp<BnFr>::mul(a, b); memcpy(rs, &a, 32);
         fr_from_mont_bytes<BnFr>(rs, rsp);
     } else {
         fr_from_mont_bytes<BlsFr>(r, rp); fr_from_mont_bytes<BlsFr>(s, sp);
-        Fp<BlsFr> a, b; memcpy(&a, r, 32); memcpy(&b, s, 32); a = Fp<BlsFr>::mul(a, b); if (negate_rs) a = Fp<BlsFr>::neg(a); memcpy(rs, &a, 32);
+        Fp<BlsFr> a, b; memcpy(&a, r, 32); memcpy(&b, s, 32); a = Fp<BlsFr>::mul(a, b); memcpy(rs, &a, 32);
         fr_from_mont_bytes<BlsFr>(rs, rsp);
     }
 }
-static int groth16_assemble_host(int curve, const GroupOps& G1, const GroupOps& G2, const VkPoints& vk, const uint8_t* partials,
-                                 const uint8_t r[32], const uint8_t s[32], uint8_t* proof);
-static int groth16_assemble(sb_ctx* c, Groth16Key* k, const uint8_t* partials, const uint8_t r[32], const uint8_t s[32], uint8_t* proof) {
-    VkPoints vk{k->alpha1.data(), k->beta1.data(), k->beta2.data(), k->delta1.data(), k->delta2.data()};
-    return groth16_assemble_host(c->curve, c->g1, c->g2, vk, partials, r, s, proof);
-}
-static int groth16_assemble_host(int curve, const GroupOps& G1, const GroupOps& G2, const VkPoints& vk, const uint8_t* partials,
-                                 const uint8_t r[32], const uint8_t s[32], uint8_t* proof) {
-    const uint32_t x1 = G1.xyzz_bytes, x2 = G2.xyzz_bytes;
-    std::vector<uint8_t> A(partials, partials + x1), B1(partials + x1, partials + 2 * x1), C(partials + 2 * x1, partials + 3 * x1),
-        H(partials + 3 * x1, partials + 4 * x1), B2(partials + 4 * x1, partials + 4 * x1 + x2);
-    uint8_t rp[32], sp[32], rsp[32];
-    plain_scalars(curve, r, s, rp, sp, rsp, true);
-    std::vector<uint8_t> t1(x1), t2(x2), d1(x1), d2(x2), pt(x1), pt2(x2);
-    G1.from_affine(vk.delta1, d1.data()); G2.from_affine(vk.delta2, d2.data());
-    // pi_a = A + alpha1 + r*delta1
-    G1.from_affine(vk.alpha1, pt.data()); G1.add(A.data(), pt.data());
-    G1.times(d1.data(), rp, 32, t1.data()); G1.add(A.data(), t1.data());
-    // pi_b = B2 + beta2 + s*delta2
-    G2.from_affine(vk.beta2, pt2.data()); G2.add(B2.data(), pt2.data());
-    G2.times(d2.data(), sp, 32, t2.data()); G2.add(B2.data(), t2.data());
-    // pib1 = B1 + beta1 + s*delta1
-    G1.from_affine(vk.beta1, pt.data()); G1.add(B1.data(), pt.data());
-    G1.times(d1.data(), sp, 32, t1.data()); G1.add(B1.data(), t1.data());
-    // pi_c = C + H + s*pi_a + r*pib1 - rs*delta1
-    G1.add(C.data(), H.data());
-    G1.times(A.data(), sp, 32, t1.data()); G1.add(C.data(), t1.data());
-    G1.times(B1.data(), rp, 32, t1.data()); G1.add(C.data(), t1.data());
-    G1.times(d1.data(), rsp, 32, t1.data()); G1.add(C.data(), t1.data());
-    G1.to_affine(A.data(), proof);
-    G2.to_affine(B2.data(), proof + G1.aff_bytes);
-    G1.to_affine(C.data(), proof + G1.aff_bytes + G2.aff_bytes);
-    return 0;
-}
 
-// The same assembly split so that nothing but three additions and three normalisations follows the last MSM:
+// The assembly is split so that nothing but three additions and three normalisations follows the last MSM:
 //   pi_a = A + [alpha1 + r*delta1],  pi_b = B2 + [beta2 + s*delta2],
 //   pi_c = C + H + s*pi_a + r*pib1 - rs*delta1 = [C + H + s*A + r*B1] + [s*alpha1 + r*beta1 + rs*delta1]
 // The bracketed fixed parts depend only on the key and (r, s): a helper thread computes them while the GPU works;
-// the C bracket is folded by groth16_device (ProofScalars) as A and B1 land.  Same group elements, same proof bytes.
+// the C bracket is folded (groth16_fold) by groth16_device as A and B1 land, or per proof on the host.
 struct FixedParts { std::vector<uint8_t> Fa, Fb, Fc; };
 // g2_thread: the G2 multiple runs on a thread of its own (a single proof's latency); false runs it in place (batch pool)
 static FixedParts groth16_fixed_parts(int curve, const GroupOps& G1, const GroupOps& G2, const VkPoints vk, const uint8_t* r, const uint8_t* s,
                                       bool g2_thread = true) {
     const uint32_t x1 = G1.xyzz_bytes, x2 = G2.xyzz_bytes;
     uint8_t rp[32], sp[32], rsp[32];
-    plain_scalars(curve, r, s, rp, sp, rsp, false);
+    plain_scalars(curve, r, s, rp, sp, rsp);
     FixedParts f; f.Fa.assign(x1, 0); f.Fb.assign(x2, 0); f.Fc.assign(x1, 0);
     std::vector<uint8_t> a1(x1), b1(x1), d1(x1), b2(x2), d2(x2), t1(x1), t2(x2);
     G1.from_affine(vk.alpha1, a1.data()); G1.from_affine(vk.beta1, b1.data()); G1.from_affine(vk.delta1, d1.data());
@@ -1464,13 +1486,29 @@ static void groth16_finish_folded(const GroupOps& G1, const GroupOps& G2, const 
     G2.to_affine(B2.data(), proof + G1.aff_bytes);
     G1.to_affine(C.data(), proof + G1.aff_bytes + G2.aff_bytes);
 }
-static int groth16_prove_folded(sb_ctx* c, Groth16Key* k, const uint8_t* witness, uint64_t n_witness, const uint8_t r[32], const uint8_t s[32], uint8_t* proof) {
+// The proof from the partials of n_shards shards (n_shards x (A | B1 | C | H | B2), XYZZ bytes): their sums, folded and
+// finished as above.
+static void groth16_assemble_host(int curve, const GroupOps& G1, const GroupOps& G2, const VkPoints& vk, const uint8_t* all, int n_shards,
+                                  const uint8_t r[32], const uint8_t s[32], uint8_t* proof) {
+    const uint32_t x1 = G1.xyzz_bytes, pb = 4 * x1 + G2.xyzz_bytes;
+    std::vector<uint8_t> acc(pb, 0);
+    for (int i = 0; i < n_shards; i++) {
+        const uint8_t* p = all + (size_t)i * pb;
+        for (int j = 0; j < 4; j++) G1.add(acc.data() + j * x1, p + j * x1);
+        G2.add(acc.data() + 4 * x1, p + 4 * x1);
+    }
+    ProofScalars ps; uint8_t rsp[32]; plain_scalars(curve, r, s, ps.rp, ps.sp, rsp);
+    groth16_fold_scalars(G1, acc.data(), ps);
+    groth16_finish_folded(G1, G2, groth16_fixed_parts(curve, G1, G2, vk, r, s, false), acc.data(), proof);
+}
+static int groth16_prove_folded(sb_ctx* c, Groth16Key* k, const uint8_t* witness, uint64_t n_witness, const uint8_t r[32], const uint8_t s[32], uint8_t* proof,
+                                const void* d_witness = nullptr) {
     VkPoints vk{k->alpha1.data(), k->beta1.data(), k->beta2.data(), k->delta1.data(), k->delta2.data()};
     const int curve = c->curve; const GroupOps G1 = c->g1, G2 = c->g2;
     std::future<FixedParts> fixed = std::async(std::launch::async, [=]() { return groth16_fixed_parts(curve, G1, G2, vk, r, s); });
-    ProofScalars ps; uint8_t rsp[32]; plain_scalars(curve, r, s, ps.rp, ps.sp, rsp, false);
+    ProofScalars ps; uint8_t rsp[32]; plain_scalars(curve, r, s, ps.rp, ps.sp, rsp);
     std::vector<uint8_t> partials(sb_groth16_partials_bytes(c));
-    int rc = groth16_device(c, k, witness, n_witness, 0, 1, partials.data(), &ps, false);
+    int rc = groth16_device(c, k, witness, n_witness, 0, 1, partials.data(), &ps, false, d_witness);
     FixedParts f = fixed.get();
     if (rc) return rc;
     groth16_finish_folded(c->g1, c->g2, f, partials.data(), proof);
@@ -1478,11 +1516,11 @@ static int groth16_prove_folded(sb_ctx* c, Groth16Key* k, const uint8_t* witness
 }
 
 // ---------------------------------------------------------------------------------------------------- Groth16 batches
-// sb_groth16_prove_batch: K proofs against one key, sub-batch by sub-batch.  A sub-batch of K' proofs runs the single-proof
-// pipeline once with K' times the work per launch: one QAP launch over K' witnesses, one strided NTT batch of 3K'
-// transforms per pass, one joinABC over K'n elements, one sort of the K' witnesses' digits (shared by A, B1, B2 and C) and
-// one of the K' H-scalar vectors, five bucket pipelines whose windows are the K' proofs' windows side by side
-// (MsmGeom::K), one download of the window sums.  Recombination and proof assembly run per proof on host threads.
+// sb_groth16_prove_batch: K proofs against one key, sub-batch by sub-batch.  A sub-batch of K' proofs runs the single
+// proof's pipeline (groth16_issue) once with K' times the work per launch: one QAP launch over K' witnesses, one strided NTT
+// batch of 3K' transforms per pass, one joinABC over K'n elements, one sort of the K' witnesses' digits (shared by A, B1, B2
+// and C) and one of the K' H-scalar vectors, five bucket pipelines whose windows are the K' proofs' windows side by side
+// (MsmGeom::K), five downloads of the window sums.  Recombination and proof assembly run per proof on host threads.
 
 // What one more proof of a sub-batch costs in device memory: its witness, six n-element arrays (the 3n transform data and
 // its 3n scratch; the H scalars reuse the scratch), the sorted entries of its witness and H digits, and its share of the
@@ -1498,22 +1536,19 @@ static size_t groth16_batch_footprint(const sb_ctx* c, const Groth16Key* k, cons
 
 // Keys whose witness or H side is longer than one MSM chunk (2^23 points, sb_set_tuning(6) lowers it): the batched sort
 // would hold every entry of a proof at once, so each proof goes through the single-proof path, which cuts its MSMs into
-// chunks.  That path uploads to the key's resident witness buffer: the resident witness is saved first and put back after.
+// chunks.  Each witness goes to the batch's witness buffer, so the resident witness is not touched.
 static int groth16_prove_batch_chunked(sb_ctx* c, Groth16Key* k, const uint8_t* witnesses, uint32_t count,
                                        const uint8_t* r, const uint8_t* s, uint8_t* proofs) {
     const uint64_t nv = k->nVars;
     const uint32_t proof_bytes = 2 * c->g1.aff_bytes + c->g2.aff_bytes;
-    const bool had = k->witness_resident;
-    void* saved = had ? k->batchW.get(nv * 32) : nullptr;
-    if (had && !saved) return fail(c, SB_ERR_NOMEM, "out of device memory (resident witness copy)");
+    void* dW = k->batchW.get(nv * 32);
+    if (!dW) return fail(c, SB_ERR_NOMEM, "out of device memory (Groth16 batch witness)");
     tick(c, 5);
-    if (had) CU(c, cudaMemcpyAsync(saved, k->dW, nv * 32, cudaMemcpyDeviceToDevice, c->stream));
-    int rc = 0;
-    for (uint32_t i = 0; i < count && !rc; i++)
-        rc = groth16_prove_folded(c, k, witnesses + (size_t)i * nv * 32, nv, r + 32 * (size_t)i, s + 32 * (size_t)i, proofs + (size_t)i * proof_bytes);
-    if (had) { CU(c, cudaMemcpyAsync(k->dW, saved, nv * 32, cudaMemcpyDeviceToDevice, c->stream)); CU(c, cudaStreamSynchronize(c->stream)); }
-    k->witness_resident = had;
-    if (rc) return rc;
+    for (uint32_t i = 0; i < count; i++) {
+        CU(c, h2d(c, dW, witnesses + (size_t)i * nv * 32, nv * 32));
+        int rc = groth16_prove_folded(c, k, nullptr, nv, r + 32 * (size_t)i, s + 32 * (size_t)i, proofs + (size_t)i * proof_bytes, dW);
+        if (rc) return rc;
+    }
     tick(c, 6);
     CU(c, cudaEventSynchronize(c->ev[6]));
     c->last_ms[0] = elapsed(c, 5, 6);
@@ -1547,99 +1582,31 @@ static int groth16_prove_batch_impl(sb_ctx* c, Groth16Key* k, const uint8_t* wit
     int rc;
     tick(c, 0);
     prof_begin(c);
-    cudaStream_t s0 = c->stream, sN = c->aux[5];
     for (uint32_t k0 = 0; k0 < count; k0 += KB) {
         const uint32_t kb = std::min(KB, count - k0);
-        MsmGeom gwK = gw, ghK = gh; gwK.K = kb; ghK.K = kb;
         const size_t tn = (size_t)kb * n * 32;   // bytes of one of A, B, C over the sub-batch
         uint8_t* dW = (uint8_t*)k->batchW.get((size_t)kb * nv * 32);
         uint8_t* X = (uint8_t*)k->batchX.get(3 * tn);
         uint8_t* Y = (uint8_t*)k->batchY.get(3 * tn);
         if (!dW || !X || !Y) return fail(c, SB_ERR_NOMEM, "out of device memory (Groth16 batch of " + std::to_string(kb) + " proofs)");
         CU(c, h2d(c, dW, witnesses + (size_t)k0 * nv * 32, (size_t)kb * nv * 32));
-        CU(c, cudaEventRecord(c->pev[0], s0));
-        CU(c, cudaStreamWaitEvent(sN, c->pev[0], 0));
-        // side stream: QAP rows -> iNTT -> coset NTT (1/n folded in) -> joinABC -> sort of the H scalars
-        { ProfScope pq(&c->stats, PROF_QAP, sN);
-          rc = fr_qap_rows(cv, k->d_rowptr, k->d_sig, k->d_coef, dW, nv, X, X + tn, X + 2 * tn, n, kb, sN); c->launches++;
-          pq.end(); }
-        if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_qap_rows");
-        const uint8_t* inc = (k->power == c->fr_s) ? c->shift.data() : c->roots[k->power + 1].data();
-        uint8_t ninv[32];
-        if (cv == SB_BN254) ninv_bytes<BnFr>(k->power, ninv); else ninv_bytes<BlsFr>(k->power, ninv);
-        FrPre fpre; rc = get_pre(c, n, ninv, inc, &fpre); if (rc) return rc;
-        FrNttTables tbi, tbf;
-        rc = get_ntt_tab(c, k->power, true, &tbi); if (rc) return rc;
-        rc = get_ntt_tab(c, k->power, false, &tbf); if (rc) return rc;
-        int side = 0, side2 = 0, launches = 0;
-        ProfScope pn(&c->stats, PROF_NTT, sN);
-        rc = fr_ntt_strided(cv, X, Y, 3 * (int)kb, k->power, &tbi, nullptr, nullptr, sN, &side, &launches);
-        if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_ntt_strided");
-        uint8_t* src = side ? Y : X; uint8_t* dst = side ? X : Y;
-        rc = fr_ntt_strided(cv, src, dst, 3 * (int)kb, k->power, &tbf, &fpre, nullptr, sN, &side2, &launches);
-        if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_ntt_strided");
-        pn.end();
-        c->launches += launches;
-        uint8_t* ev = side2 ? dst : src; uint8_t* hsc = side2 ? src : dst;   // coset evaluations; the H scalars go to the other half
-        { ProfScope pj(&c->stats, PROF_JOIN, sN);
-          rc = fr_join_abc(cv, ev, ev + tn, ev + 2 * tn, hsc, (uint64_t)kb * n, sN); c->launches++;
-          pj.end(); }
-        if (rc) return cuda_fail(c, (cudaError_t)rc, "fr_join_abc");
-        MsmSorted sh;
-        rc = msm_sort_entries(hsc, 32, n, ghK, c->sort_scratch2, sN, &sh, &c->stats);
-        if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
-        CU(c, cudaEventRecord(c->pev[1], sN));
-        // main stream: the witness digits, sorted once for A, B1, B2 and C
-        MsmSorted sw;
-        rc = msm_sort_entries(dW, 32, nv, gwK, c->sort_scratch, s0, &sw, &c->stats);
-        if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
-        const size_t w1 = (size_t)gwK.wsum_points() * x1, w2 = (size_t)gwK.wsum_points() * x2, wh = (size_t)ghK.wsum_points() * x1;
-        const size_t wtot = 3 * w1 + w2 + wh;
-        rc = groth16_wsum_room(c, k, wtot, wtot + 64);
+        Groth16Jobs t;
+        rc = groth16_issue(c, k, dW, kb, 0, nv, 0, n, false, &t);
         if (rc) return rc;
-        uint8_t* dws = (uint8_t*)k->dWsum; uint8_t* hws = c->pinned;
-        uint64_t* hcounts = (uint64_t*)(c->pinned + wtot);
-        struct Job { const GroupOps* G; const void* bases; size_t off; size_t len; int tag; const MsmSorted* srt; };
-        const Job jobs[5] = {{&G1, pre ? k->tA : k->dA, 0, w1, SB_G1, &sw},
-                             {&G1, pre ? k->tB1 : k->dB1, w1, w1, SB_G1, &sw},
-                             {&G2, pre ? k->tB2 : k->dB2, 3 * w1, w2, SB_G2, &sw},
-                             {&G1, pre ? k->tC : k->dC, 2 * w1, w1, SB_G1, &sw},
-                             {&G1, pre ? k->tH : k->dH, 3 * w1 + w2, wh, SB_G1, &sh}};
+        // the pinned area serves the next sub-batch: the host work gets its own copy, taken job by job as each lands, and
+        // runs while the GPU goes on
+        auto host = std::make_shared<std::vector<uint8_t>>(t.job[4].off + t.job[4].len);
         for (int i = 0; i < 5; i++) {
-            cudaStream_t st = c->aux[i];
-            if (i == 4) CU(c, cudaStreamWaitEvent(s0, c->pev[1], 0));   // H needs the NTT chain
-            c->stats.cur_tag = jobs[i].tag;
-            rc = jobs[i].G->buckets(jobs[i].bases, *jobs[i].srt, c->bscr[i], s0, dws + jobs[i].off, &c->stats, st, c->pev[8 + i]);
-            if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_buckets");
-            CU(c, cudaMemcpyAsync(hws + jobs[i].off, dws + jobs[i].off, jobs[i].len, cudaMemcpyDeviceToHost, st));
-            if (i == 0) CU(c, cudaMemcpyAsync(&hcounts[0], sw.counts, 8, cudaMemcpyDeviceToHost, st));
-            if (i == 4) CU(c, cudaMemcpyAsync(&hcounts[1], sh.counts, 8, cudaMemcpyDeviceToHost, st));
-            CU(c, cudaEventRecord(c->pev[2 + i], st));
+            CU(c, cudaEventSynchronize(c->pev[2 + i]));
+            memcpy(host->data() + t.job[i].off, c->pinned + t.job[i].off, t.job[i].len);
         }
-        for (int i = 0; i < 5; i++) { CU(c, cudaEventSynchronize(c->pev[2 + i])); CU(c, cudaStreamWaitEvent(s0, c->pev[2 + i], 0)); }
-        c->stat[4] += 3.0 * (double)hcounts[0] + (double)hcounts[1]; c->stat[5] += (double)hcounts[0];
-        // the pinned area serves the next sub-batch: the host work gets its own copy and runs while the GPU goes on.
-        // Proof q's window sums start q * windows_per_proof * msm_wsum_parts points into each MSM's region.
-        auto host = std::make_shared<std::vector<uint8_t>>(hws, hws + wtot);
-        const size_t sw1 = (size_t)msm_wsum_parts(gw) * gw.windows_per_proof(), swh = (size_t)msm_wsum_parts(gh) * gh.windows_per_proof();
-        size_t offs[5];
-        const size_t per[5] = {sw1 * x1, sw1 * x1, sw1 * x2, sw1 * x1, swh * x1};
-        for (int i = 0; i < 5; i++) offs[i] = jobs[i].off;
-        for (uint32_t p = k0; p < k0 + kb; p++) pool.submit([&, host, p, k0, offs, per]() {
+        t.tally(c);
+        for (uint32_t p = k0; p < k0 + kb; p++) pool.submit([&, host, t, p, k0]() {
             const size_t q = p - k0;
-            const uint8_t* ws = host->data();
-            uint8_t* pA = allp.data() + (size_t)p * pb; uint8_t* pB1 = pA + x1; uint8_t* pC = pB1 + x1; uint8_t* pH = pC + x1; uint8_t* pB2 = pH + x1;
-            G1.combine(ws + offs[0] + q * per[0], gw, pA);
-            G1.combine(ws + offs[1] + q * per[1], gw, pB1);
-            G2.combine(ws + offs[2] + q * per[2], gw, pB2);
-            G1.combine(ws + offs[3] + q * per[3], gw, pC);
-            G1.combine(ws + offs[4] + q * per[4], gh, pH);
-            // C' = C + H + s*A + r*B1, as groth16_device folds it
-            ProofScalars ps; uint8_t rsp[32]; plain_scalars(cv, r + 32 * (size_t)p, s + 32 * (size_t)p, ps.rp, ps.sp, rsp, false);
-            std::vector<uint8_t> t(x1);
-            G1.add(pC, pH);
-            G1.times(pA, ps.sp, 32, t.data()); G1.add(pC, t.data());
-            G1.times(pB1, ps.rp, 32, t.data()); G1.add(pC, t.data());
+            uint8_t* part = allp.data() + (size_t)p * pb;
+            for (const Groth16Job& j : t.job) j.G->combine(host->data() + j.off + q * j.per, j.g, part + j.part);
+            ProofScalars ps; uint8_t rsp[32]; plain_scalars(cv, r + 32 * (size_t)p, s + 32 * (size_t)p, ps.rp, ps.sp, rsp);
+            groth16_fold_scalars(G1, part, ps);
         });
     }
     pool.wait();   // every fixed part and every folded partial
@@ -1682,15 +1649,9 @@ int sb_groth16_prove_shard(sb_ctx* c, uint64_t h, const uint8_t* witness, uint64
 }
 int sb_groth16_finish(sb_ctx* c, uint64_t h, const uint8_t* all, int n_shards, const uint8_t r[32], const uint8_t s[32], uint8_t* proof) { SB_LOCK(c);
     Groth16Key* k = get_key(c, h); if (!k) return fail(c, SB_ERR_ARG, "invalid groth16 handle");
-    const GroupOps& G1 = c->g1; const GroupOps& G2 = c->g2;
-    const uint32_t x1 = G1.xyzz_bytes, pb = sb_groth16_partials_bytes(c);
-    std::vector<uint8_t> acc(pb, 0);
-    for (int i = 0; i < n_shards; i++) {
-        const uint8_t* p = all + (size_t)i * pb;
-        for (int j = 0; j < 4; j++) G1.add(acc.data() + j * x1, p + j * x1);
-        G2.add(acc.data() + 4 * x1, p + 4 * x1);
-    }
-    return groth16_assemble(c, k, acc.data(), r, s, proof);
+    const VkPoints vk{k->alpha1.data(), k->beta1.data(), k->beta2.data(), k->delta1.data(), k->delta2.data()};
+    groth16_assemble_host(c->curve, c->g1, c->g2, vk, all, n_shards, r, s, proof);
+    return 0;
 }
 
 // One proof across the ranks of a communicator (collective: every rank calls it with the same witness, r and s).
@@ -1705,7 +1666,7 @@ int sb_groth16_prove_dist(sb_ctx* c, uint64_t h, const uint8_t* witness, uint64_
     const int curve = c->curve; const GroupOps G1 = c->g1, G2 = c->g2;
     std::future<FixedParts> fixed;
     if (proof) fixed = std::async(std::launch::async, [=]() { return groth16_fixed_parts(curve, G1, G2, vk, r, s); });
-    ProofScalars ps; uint8_t rsp[32]; plain_scalars(curve, r, s, ps.rp, ps.sp, rsp, false);
+    ProofScalars ps; uint8_t rsp[32]; plain_scalars(curve, r, s, ps.rp, ps.sp, rsp);
     const size_t pb = sb_groth16_partials_bytes(c);
     uint8_t* mine = c->h_xchg + pb * c->world;
     int rc = groth16_device(c, k, witness, n_witness, c->rank, c->world, mine, &ps, true);
@@ -1796,15 +1757,9 @@ int sb_host_groth16_finish(int curve, const uint8_t* vk_alpha1, const uint8_t* v
                            const uint8_t r[32], const uint8_t s[32], uint8_t* proof_affine_out) {
     if ((curve != SB_BN254 && curve != SB_BLS12_381) || n_shards < 1) return SB_ERR_ARG;
     GroupOps G1, G2; host_ops(curve, G1, G2);
-    const uint32_t x1 = G1.xyzz_bytes, pb = 4 * G1.xyzz_bytes + G2.xyzz_bytes;
-    std::vector<uint8_t> acc(pb, 0);
-    for (int i = 0; i < n_shards; i++) {
-        const uint8_t* p = partials_all_ranks + (size_t)i * pb;
-        for (int j = 0; j < 4; j++) G1.add(acc.data() + j * x1, p + j * x1);
-        G2.add(acc.data() + 4 * x1, p + 4 * x1);
-    }
-    VkPoints vk{vk_alpha1, vk_beta1, vk_beta2, vk_delta1, vk_delta2};
-    return groth16_assemble_host(curve, G1, G2, vk, acc.data(), r, s, proof_affine_out);
+    const VkPoints vk{vk_alpha1, vk_beta1, vk_beta2, vk_delta1, vk_delta2};
+    groth16_assemble_host(curve, G1, G2, vk, partials_all_ranks, n_shards, r, s, proof_affine_out);
+    return 0;
 }
 // point range of shard `shard` of `n_shards` over `total` points (the split sb_groth16_prove_shard uses)
 void sb_shard_range(uint64_t total, int shard, int n_shards, uint64_t* first, uint64_t* count) {

@@ -129,9 +129,9 @@ def test_shape_batches_equal_oracle(curves, label):
 
 # (1, 1) and c = 22 (2^21 buckets per window, beyond the axis-sum design) take the running-sum reduction, which returns one
 # window sum per window instead of five parts; (6, 8) cuts MSMs into 256-point chunks, which sends the 2^12 keys through
-# the single-proof path proof by proof (the 2^6 key stays batched).
+# the single-proof path proof by proof (the 2^6 key stays batched); (2, 1) runs every stream serialised on one.
 MODES = {"no_tables": [(3, 1)], "c3": [(13, 3)], "c8": [(13, 8)], "c16": [(13, 16)], "c22": [(13, 22)],
-         "force_reduce": [(1, 1)], "chunked": [(6, 8)], "split1": [(14, 1)], "split3": [(14, 3)]}
+         "force_reduce": [(1, 1)], "chunked": [(6, 8)], "split1": [(14, 1)], "split3": [(14, 3)], "serial": [(2, 1)]}
 MODE_KEYS = [(BN, 6), (BN, 12), (BLS, 12)]
 # c = 22 without window tables (the 2^6 key) would allocate 12 windows of 2^21 buckets per MSM and proof: not run
 MODE_CASES = [(cid, L, m) for cid, L in MODE_KEYS for m in MODES if not (L == 6 and m == "c22")]
@@ -186,7 +186,7 @@ def test_resident_witness_and_errors(curves):
         assert pk.prove_batch_raw(np.zeros(0, np.uint8), []) == []
     finally:
         pk.release()
-    # the per-proof path of keys longer than one MSM chunk saves and restores the resident witness
+    # the per-proof path of keys longer than one MSM chunk does not touch the resident witness
     with tuning(c.lib, [(6, 8)]):
         pk = load(curves, cid, zkey)
         try:
