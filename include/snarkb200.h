@@ -180,6 +180,21 @@ uint32_t sb_fflonk_proof_bytes(sb_ctx* ctx);
 int sb_fflonk_prove_resident(sb_ctx* ctx, uint64_t handle, const uint8_t* blinders, uint8_t* proof_out);
 int sb_fflonk_prove(sb_ctx* ctx, uint64_t handle, const uint8_t* witness, uint64_t n_witness, const uint8_t* blinders,
                     uint8_t* proof_out);
+/* count fflonk proofs against one loaded key, with the contract of sb_plonk_prove_batch: witnesses = count * n_witness * 32
+ * bytes; blinders = count * 9 * 32 bytes (b_1..b_9 per proof, Montgomery); proofs_out = count * sb_fflonk_proof_bytes();
+ * status_out = count int32 (may be NULL).  Proof k is byte-identical to sb_fflonk_prove(witness k, blinders k).  The proofs
+ * run in lockstep in sub-batches sized from free device memory (sb_set_tuning(14) caps them).
+ * - Argument errors come before any device work, as for sb_plonk_prove_batch.
+ * - A proof the reference would reject does not stop the others.  Its slot is zero-filled and status_out[k] holds the code of
+ *   its first error: 3 "Copy constraints does not match", 4 "Polynomial is not divisible", 5 "T0 Polynomial is not well
+ *   calculated", 6 "T1 ...", 7 "T2 ...", 8 "Degree of L(X)/(ZTS2(y)(X-y)) remainder should be 0"; 0 for a good proof.  The call
+ *   then returns SB_ERR_ARG, and sb_last_error holds the text of the lowest-index failing proof.  Keys with nPublic = 0
+ *   prove, as with sb_fflonk_prove.
+ * - The batch's device buffers grow with the largest sub-batch and belong to the key (sb_fflonk_release frees them).  When
+ *   not even one proof fits, the call fails with SB_ERR_NOMEM and says how much one proof needs.
+ * - The resident witness of sb_fflonk_prove_resident is left as it was.  sb_last_ms(0) = the whole call. */
+int sb_fflonk_prove_batch(sb_ctx* ctx, uint64_t handle, const uint8_t* witnesses, uint64_t n_witness, uint32_t count,
+                          const uint8_t* blinders, uint8_t* proofs_out, int32_t* status_out);
 int sb_fflonk_release(sb_ctx* ctx, uint64_t handle);
 /* multi-GPU: this rank proves with its shard [shard, n_shards) of every MSM and returns the five un-normalised
  * MSM partials (A, B1, C, H in G1; B2 in G2) instead of a proof; the ranks exchange them (NCCL all-gather) and any
@@ -258,7 +273,7 @@ double sb_calibrate(sb_ctx* ctx, int what);
  *      is chosen: per chunk for MSMs on unregistered bases, and for window tables when they are built, i.e. when bases are
  *      registered or a key is loaded; a table keeps the c in force at that moment.  Tables are still skipped when
  *      W * n >= 2^31.  A large c costs memory: a plain MSM allocates W * 2^(c-1) buckets.
- *  14  most proofs per sub-batch of sb_groth16_prove_batch and sb_plonk_prove_batch, and rows per sub-batch of
+ *  14  most proofs per sub-batch of sb_groth16_prove_batch, sb_plonk_prove_batch and sb_fflonk_prove_batch, and rows per sub-batch of
  *      sb_msm_registered_batch (test hook;
  *      0 = default: as many as the 32-bit bucket keys and free device memory allow)
  * The Python mirror applies SB_TUNE="key=value,..." from the environment when it loads the library. */

@@ -64,6 +64,7 @@ _SIGNATURES = {
     "sb_fflonk_proof_bytes": (u32, [vp]),
     "sb_fflonk_prove": (ctypes.c_int, [vp, u64, vp, u64, ctypes.c_char_p, vp]),
     "sb_fflonk_prove_resident": (ctypes.c_int, [vp, u64, ctypes.c_char_p, vp]),
+    "sb_fflonk_prove_batch": (ctypes.c_int, [vp, u64, vp, u64, u32, vp, vp, vp]),
     "sb_fflonk_release": (ctypes.c_int, [vp, u64]),
     "sb_groth16_prove_resident": (ctypes.c_int, [vp, u64, vp, vp, vp]),
     "sb_last_stat": (ctypes.c_double, [vp, ctypes.c_int]),

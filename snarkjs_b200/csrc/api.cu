@@ -1875,6 +1875,16 @@ int sb_fflonk_prove_resident(sb_ctx* c, uint64_t h, const uint8_t* blinders, uin
     cudaSetDevice(c->device);
     return fflonk_prove_impl<BnFq, BnFr>(c, k, nullptr, 0, blinders, proof);
 }
+int sb_fflonk_prove_batch(sb_ctx* c, uint64_t h, const uint8_t* witnesses, uint64_t n_witness, uint32_t count, const uint8_t* blinders,
+                          uint8_t* proofs, int32_t* status) { SB_LOCK(c);
+    FflonkKeyDev* k = get_fflonk_key(c, h); if (!k) return fail(c, SB_ERR_ARG, "invalid fflonk handle");
+    if (n_witness != (uint64_t)k->z.nVars - k->z.nAdditions)                                          // fflonk_prove.js:79-81
+        return fail(c, SB_ERR_ARG, "Invalid witness length. Circuit: " + std::to_string(k->z.nVars) + ", witness: " + std::to_string(n_witness) + ", " + std::to_string(k->z.nAdditions));
+    if (count == 0) return SB_OK;
+    if (!witnesses || !blinders || !proofs) return fail(c, SB_ERR_ARG, "null argument");
+    cudaSetDevice(c->device);
+    return fflonk_prove_batch_impl<BnFq, BnFr>(c, k, witnesses, n_witness, count, blinders, proofs, status);
+}
 int sb_fflonk_release(sb_ctx* c, uint64_t h) { SB_LOCK(c);
     FflonkKeyDev* k = get_fflonk_key(c, h); if (!k) return fail(c, SB_ERR_ARG, "invalid fflonk handle");
     cudaSetDevice(c->device); cudaStreamSynchronize(c->stream);

@@ -90,6 +90,34 @@ class ProvingKey:
             c.check(lib.sb_fflonk_prove(c.handle, self.handle, _ptr(w), w.size // 32, bytes(blinders), _ptr(out)))
         return out.tobytes()
 
+    def prove_batch_raw(self, witnesses, blinders_list) -> list:
+        """One sb_fflonk_prove_batch call: witnesses = wtns section-2 payloads ((nVars - nAdditions) x 32 bytes each),
+        blinders_list = one 9 x 32-byte Montgomery blinder string per witness.  Returns one proof (bytes, as prove_raw) per
+        witness, or None for a proof the reference would have rejected; raises SbError for argument and device errors."""
+        parts = [_arr(x) for x in witnesses]
+        count = len(parts)
+        if len(blinders_list) != count:
+            raise SbError("one blinder set per witness")
+        if count == 0:
+            return []
+        for b in blinders_list:
+            if len(b) != 9 * 32:
+                raise SbError("blinders must be 9 field elements")
+        n_wit = parts[0].size // 32
+        for x in parts:
+            if x.size != parts[0].size:
+                raise SbError("witnesses of one batch must have the same length")
+        lib, c = self.curve.lib, self.curve
+        w = np.concatenate(parts)
+        bl = np.frombuffer(b"".join(bytes(b) for b in blinders_list), np.uint8)
+        pb = lib.sb_fflonk_proof_bytes(c.handle)
+        out = np.empty(count * pb, np.uint8)
+        status = np.zeros(count, np.int32)
+        rc = lib.sb_fflonk_prove_batch(c.handle, self.handle, _ptr(w), n_wit, count, _ptr(bl), _ptr(out), _ptr(status))
+        if rc != 0 and not status.any():
+            c.check(rc)
+        return [None if status[i] else out[i * pb:(i + 1) * pb].tobytes() for i in range(count)]
+
     def release(self):
         if self.handle:
             self.curve.lib.sb_fflonk_release(self.curve.handle, self.handle)
@@ -110,6 +138,36 @@ def prove(zkey, wtns: bytes, blinders: bytes | None = None, logger=None, options
         raw = pk.prove_raw(np.frombuffer(W, np.uint8), blinders)
         pub = [str(int.from_bytes(W[i * 32:(i + 1) * 32], "little")) for i in range(1, pk.nPublic + 1)]
         return proof_to_object(pk.curve, raw), pub
+    finally:
+        if not isinstance(zkey, ProvingKey):
+            pk.release()
+
+
+def prove_batch(zkey, wtns_list, blinders=None):
+    """fflonkProve over many witnesses of one circuit in one device call: [(proof, publicSignals), ...] in the order of
+    wtns_list.  zkey may be bytes or a ProvingKey; every .wtns container is checked as prove checks it; blinders = one
+    9 x 32-byte Montgomery string per witness, drawn like Fr.random() when not given.  A witness the reference would
+    reject raises SbError with the reference's text for the first such witness."""
+    pk = zkey if isinstance(zkey, ProvingKey) else ProvingKey(zkey)
+    try:
+        ws = []
+        for wtns in wtns_list:
+            wh, W = read_wtns_header(bytes(wtns))
+            if wh["q"] != pk.header["r"]:
+                raise SbError("Curve of the witness does not match the curve of the proving key")          # :75-77
+            ws.append(W)
+        if blinders is None:
+            blinders = [b"".join(random_fr(pk.curve) for _ in range(9)) for _ in ws]                      # :321-324
+        if len(blinders) != len(ws):
+            raise SbError("one blinder set per witness")
+        raws = pk.prove_batch_raw([np.frombuffer(W, np.uint8) for W in ws], blinders)                   # length check in C (:79-81)
+        if any(r is None for r in raws):
+            raise SbError(pk.curve.lib.sb_last_error(pk.curve.handle).decode())
+        out = []
+        for W, raw in zip(ws, raws):
+            pub = [str(int.from_bytes(W[i * 32:(i + 1) * 32], "little")) for i in range(1, pk.nPublic + 1)]
+            out.append((proof_to_object(pk.curve, raw), pub))
+        return out
     finally:
         if not isinstance(zkey, ProvingKey):
             pk.release()
