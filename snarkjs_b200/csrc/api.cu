@@ -104,7 +104,7 @@ struct sb_ctx {
     GroupOps g1, g2;
     MsmScratch sort_scratch, bucket_scratch;
     MsmScratch sort_scratch2, bscr[5];           // per-MSM scratch for the overlapped Groth16 pipeline
-    cudaStream_t aux[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // high-priority side streams (tails, NTT chain)
+    cudaStream_t aux[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // side streams (tails, NTT chain), the main stream's priority
     cudaEvent_t pev[16];                         // pipeline events
     uint8_t* pinned = nullptr;                   // pinned staging of a Groth16 proof's window sums and counters: 256 KiB,
     size_t pinned_bytes = 0;                     // grown by groth16_wsum_room when a geometry needs more
@@ -512,8 +512,11 @@ int sb_create(int curve, int device_id, sb_ctx** out) {
     for (auto& e : c->ev) cudaEventCreate(&e);
     for (auto& e : c->prof_ev) cudaEventCreate(&e);
     for (auto& e : c->pev) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
-    { int lo = 0, hi = 0; cudaDeviceGetStreamPriorityRange(&lo, &hi);
-      for (auto& st : c->aux) cudaStreamCreateWithPriority(&st, cudaStreamDefault, hi); }
+    // The side streams take the main stream's priority: a higher one lets every latency-bound tail CTA take the SM slot
+    // of a retiring accumulation CTA ahead of the accumulation's next block, which stretches the accumulation by the
+    // tail's full length (2^20 Groth16 proof, H100 at 700 W: 41.2 proofs/s with high-priority side streams, 42.0-42.3
+    // without; DESIGN §7).  At equal priority the tails fill the slots the accumulation leaves in its last wave.
+    for (auto& st : c->aux) cudaStreamCreate(&st);
     if (cudaHostAlloc((void**)&c->pinned, 256 * 1024, cudaHostAllocDefault) != cudaSuccess) c->pinned = nullptr;
     else c->pinned_bytes = 256 * 1024;
     for (int i = 0; i < 2; i++) { if (cudaHostAlloc((void**)&c->stage[i], STAGE_BYTES, cudaHostAllocDefault) != cudaSuccess) c->stage[i] = nullptr; cudaEventCreateWithFlags(&c->stage_ev[i], cudaEventDisableTiming); }
@@ -1243,7 +1246,8 @@ static int groth16_qap_ntt(sb_ctx* c, Groth16Key* k, const void* dW, uint32_t K,
 // area (len bytes at off, proof q's at off + q * per) and the offset of its partial in a proof's A | B1 | C | H | B2.
 struct Groth16Job { const GroupOps* G; MsmGeom g; size_t off, len, per, part; };
 struct Groth16Jobs {
-    Groth16Job job[5];        // A, B1, B2, C, H: the order they are issued and land in; H's region ends the area
+    enum { B2, A, B1, C, H };
+    Groth16Job job[5];        // B2, A, B1, C, H: the order they are issued and land in; H's region ends the area
     const uint64_t* counts;   // pinned: the sorted entries of the witness and of the H digits
     // sb_last_stat 4 and 5, once every job has landed
     void tally(sb_ctx* c) const { c->stat[4] += 3.0 * (double)counts[0] + (double)counts[1]; c->stat[5] += (double)counts[0]; }
@@ -1252,11 +1256,13 @@ struct Groth16Jobs {
 // The device work of K proofs (witness q at dW + q * nVars elements) over the witness points [wlo, wlo + wcnt) and the H
 // points [hlo, hlo + hcnt), each at most one MSM chunk; K > 1 only with the full ranges.  The witness is sorted once (A,
 // B1, B2 and C all multiply it, :84-97); the five bucket pipelines run on their own streams so that the latency-bound
-// tails (fold cascade, bucket reduction) of one MSM hide under the throughput-bound accumulation of the next; the H
+// tails (fold cascade, bucket reduction) of one MSM run beside the throughput-bound accumulation of the next; the H
 // scalars (QAP/NTT chain) are produced concurrently.  g_serial_prove serialises everything on one stream (profiling).
-//   main stream  : sort(witness), acc A, acc B1, acc B2, acc C, [wait for the NTT chain], acc H
-//   aux[5] (hi)  : QAP -> iNTT -> coset NTT -> [exchange] -> joinABC -> sort(H scalars)
-//   aux[0..4](hi): the tail of MSM i (fold, reduce, window sum) and its D2H into the pinned area, then pev[2 + i]
+// The G2 accumulation goes first: its CTAs (2 x 128 threads x 248 allocated registers per SM) leave no room beside
+// them, so no side work that could run beside a G1 accumulation is left waiting behind it.
+//   main stream : sort(witness), acc B2, acc A, acc B1, acc C, [wait for the NTT chain], acc H
+//   aux[5]      : QAP -> iNTT -> coset NTT -> [exchange] -> joinABC -> sort(H scalars)
+//   aux[0..4]   : the tail of job i (fold, reduce, window sum) and its D2H into the pinned area, then pev[2 + i]
 // Returns with the work queued and the main stream waiting for all of it; job i's window sums are on the host once
 // pev[2 + i] has fired.
 static int groth16_issue(sb_ctx* c, Groth16Key* k, const void* dW, uint32_t K, uint64_t wlo, uint64_t wcnt, uint64_t hlo, uint64_t hcnt,
@@ -1293,25 +1299,26 @@ static int groth16_issue(sb_ctx* c, Groth16Key* k, const void* dW, uint32_t K, u
     rc = msm_sort_entries((const uint8_t*)dW + wlo * 32, 32, wcnt, gwK, c->sort_scratch, s0, &sw, &c->stats);
     if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_sort_entries");
     tick(c, 2);
-    // A and B1 first (a single proof folds s*A + r*B1 on the host as they land), then the long G2 MSM, C, and H last
+    // the G2 MSM first, then A and B1 (a single proof folds s*A + r*B1 on the host as they land), C, and H last;
+    // window sums in the area A | B1 | C | B2 | H, partials in a proof's A | B1 | C | H | B2
     const size_t pw = (size_t)msm_wsum_parts(gw) * gw.windows_per_proof(), ph = (size_t)msm_wsum_parts(gh) * gh.windows_per_proof();
-    *out = Groth16Jobs{{{&G1, gw, 0, w1, pw * x1, 0}, {&G1, gw, w1, w1, pw * x1, x1}, {&G2, gw, 3 * w1, w2, pw * x2, 4 * x1},
+    *out = Groth16Jobs{{{&G2, gw, 3 * w1, w2, pw * x2, 4 * x1}, {&G1, gw, 0, w1, pw * x1, 0}, {&G1, gw, w1, w1, pw * x1, x1},
                         {&G1, gw, 2 * w1, w1, pw * x1, 2 * x1}, {&G1, gh, 3 * w1 + w2, wh, ph * x1, 3 * x1}}, hcounts};
-    const void* bases[5] = {pre ? k->tA : (const void*)((const uint8_t*)k->dA + wb * G1.aff_bytes),
+    const void* bases[5] = {pre ? k->tB2 : (const void*)((const uint8_t*)k->dB2 + wb * G2.aff_bytes),
+                            pre ? k->tA : (const void*)((const uint8_t*)k->dA + wb * G1.aff_bytes),
                             pre ? k->tB1 : (const void*)((const uint8_t*)k->dB1 + wb * G1.aff_bytes),
-                            pre ? k->tB2 : (const void*)((const uint8_t*)k->dB2 + wb * G2.aff_bytes),
                             pre ? k->tC : (const void*)((const uint8_t*)k->dC + wb * G1.aff_bytes),
                             pre ? k->tH : (const void*)((const uint8_t*)k->dH + hb * G1.aff_bytes)};
     for (int i = 0; i < 5; i++) {
         const Groth16Job& j = out->job[i];
         cudaStream_t st = serial ? s0 : c->aux[i];
-        if (i == 4 && sN != s0) CU(c, cudaStreamWaitEvent(s0, c->pev[1], 0));   // H needs the NTT chain
+        if (i == Groth16Jobs::H && sN != s0) CU(c, cudaStreamWaitEvent(s0, c->pev[1], 0));   // H needs the NTT chain
         c->stats.cur_tag = j.G == &G1 ? SB_G1 : SB_G2;
-        rc = j.G->buckets(bases[i], i == 4 ? sh : sw, c->bscr[i], s0, dws + j.off, &c->stats, st, c->pev[8 + i]);
+        rc = j.G->buckets(bases[i], i == Groth16Jobs::H ? sh : sw, c->bscr[i], s0, dws + j.off, &c->stats, st, c->pev[8 + i]);
         if (rc) return cuda_fail(c, (cudaError_t)rc, "msm_buckets");
         CU(c, cudaMemcpyAsync(hws + j.off, dws + j.off, j.len, cudaMemcpyDeviceToHost, st));
         if (i == 0) CU(c, cudaMemcpyAsync(&hcounts[0], sw.counts, 8, cudaMemcpyDeviceToHost, st));
-        if (i == 4) CU(c, cudaMemcpyAsync(&hcounts[1], sh.counts, 8, cudaMemcpyDeviceToHost, st));
+        if (i == Groth16Jobs::H) CU(c, cudaMemcpyAsync(&hcounts[1], sh.counts, 8, cudaMemcpyDeviceToHost, st));
         CU(c, cudaEventRecord(c->pev[2 + i], st));
     }
     tick(c, 3);
@@ -1387,8 +1394,8 @@ static int groth16_device(sb_ctx* c, Groth16Key* k, const uint8_t* witness, uint
             const Groth16Job& j = t.job[i];
             CU(c, cudaEventSynchronize(c->pev[2 + i]));
             j.G->combine(c->pinned + j.off, j.g, partials + j.part);
-            if (ps && i == 0) G1.times(pA, ps->sp, 32, sA.data());      // s * A   (src/groth16_prove.js:117: pi_c += s*pi_a)
-            if (ps && i == 1) G1.times(pB1, ps->rp, 32, rB1.data());    // r * B1  (:118)
+            if (ps && i == Groth16Jobs::A) G1.times(pA, ps->sp, 32, sA.data());      // s * A   (src/groth16_prove.js:117: pi_c += s*pi_a)
+            if (ps && i == Groth16Jobs::B1) G1.times(pB1, ps->rp, 32, rB1.data());   // r * B1  (:118)
         }
         t.tally(c);
     } else {
