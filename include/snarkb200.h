@@ -196,6 +196,33 @@ int sb_fflonk_prove(sb_ctx* ctx, uint64_t handle, const uint8_t* witness, uint64
 int sb_fflonk_prove_batch(sb_ctx* ctx, uint64_t handle, const uint8_t* witnesses, uint64_t n_witness, uint32_t count,
                           const uint8_t* blinders, uint8_t* proofs_out, int32_t* status_out);
 int sb_fflonk_release(sb_ctx* ctx, uint64_t handle);
+/* ---- one PLONK / fflonk proof on several devices, each commitment sharded over the PTau point range -------------------
+ * The rounds stay serial (the transcript needs every commitment before the next round), so rank 0 = ctxs[0] runs the whole
+ * single-device proof (kernels, NTTs, transcript, evaluations) and only the commitments are split: the P PTau points
+ * (P = n + 6 for PLONK, 9n + 18 for fflonk) go to the n contexts in the contiguous ranges sb_shard_range(P, i, n), and each
+ * commitment over `len` points is the sum of one MSM partial per rank over the part of [0, len) inside its range.  Rank 0's
+ * scalars reach the other ranks by CUDA peer copy (no NCCL; contexts from sb_create or sb_create_multi, several of them may
+ * share one device), the partials come back to the host, and the sum is normalised there: the proof is byte-identical to
+ * sb_plonk_prove / sb_fflonk_prove with the same witness and blinders.
+ * sb_*_load_multi: n in 1..64 distinct contexts; the n loads run on parallel host threads.  Rank 0 holds everything
+ *   sb_*_load holds except the PTau points outside its range; ranks i > 0 hold only their PTau range (with its window table
+ *   when the range is large enough for one) and a receive buffer of range x 32 bytes.  Ranks on different devices get peer
+ *   access to rank 0's device where the devices allow it.  If a rank fails, the handles already made are released and the
+ *   call returns that rank's code, with its message on ctxs[0].  With n = 1 the call is sb_*_load.
+ * Each handle is freed with sb_*_release(ctxs[i], handles[i]), and sb_*_info works on it.  sb_*_prove, sb_*_prove_resident
+ *   and sb_*_prove_batch refuse every handle of a multi load with n > 1 (SB_ERR_ARG): no rank holds the whole PTau.
+ * sb_*_prove_multi: handles[i] = handles_out[i] of one sb_*_load_multi call with the same contexts in the same order;
+ *   witness and blinders as for sb_*_prove.  Null pointers, n outside 1..64, a context given twice, contexts of different
+ *   curves and handles of another load, rank or order give SB_ERR_ARG before any device work; every other refusal has the
+ *   single path's code and text (witness length, copy constraints, divisibility, T checks, PLONK keys with nPublic = 0).
+ *   The call holds every context's lock for its duration.  A CUDA error on any rank is reported on ctxs[0]
+ *   (sb_last_error), and sb_last_ms(ctxs[0], 0..5) mean what they mean for sb_*_prove.  With n = 1 the call is sb_*_prove. */
+int sb_plonk_load_multi(sb_ctx* const* ctxs, int n, const uint8_t* zkey, uint64_t zkey_len, uint64_t* handles_out);
+int sb_plonk_prove_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, const uint8_t* witness, uint64_t n_witness,
+                         const uint8_t* blinders, uint8_t* proof_out);
+int sb_fflonk_load_multi(sb_ctx* const* ctxs, int n, const uint8_t* zkey, uint64_t zkey_len, uint64_t* handles_out);
+int sb_fflonk_prove_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, const uint8_t* witness, uint64_t n_witness,
+                          const uint8_t* blinders, uint8_t* proof_out);
 /* multi-GPU: this rank proves with its shard [shard, n_shards) of every MSM and returns the five un-normalised
  * MSM partials (A, B1, C, H in G1; B2 in G2) instead of a proof; the ranks exchange them (NCCL all-gather) and any
  * rank finishes with sb_groth16_finish. */

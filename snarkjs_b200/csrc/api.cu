@@ -8,6 +8,7 @@
 #include <map>
 #include <algorithm>
 #include <mutex>
+#include <atomic>
 #include <future>
 #include <thread>
 #include <functional>
@@ -1789,6 +1790,89 @@ int sb_groth16_prove_wtns(sb_ctx* c, uint64_t h, const uint8_t* w, uint64_t wlen
 #include "api_plonk.inl"
 #include "api_fflonk.inl"
 
+// ---- one PLONK / fflonk proof on several devices (sb_plonk_load_multi .. sb_fflonk_prove_multi)
+// a key of a multi load holds one PTau range only, so the single-device entries refuse it
+#define MULTI_HANDLE(proto) "this " #proto " key is one shard of sb_" #proto "_load_multi: prove with sb_" #proto "_prove_multi"
+
+// sb_*_load_multi: argument checks, then rank i's part loaded by load(ctxs[i], i, id, &handles[i]) on its own thread (under
+// that context's lock).  A rank on another device than rank 0 gets peer access to rank 0's device where the devices allow
+// it (otherwise the peer copies stage through the host).  If a rank fails, the handles made are released and rank 0's
+// context reports the failing rank's code and message.
+// Checks every sb_*_load_multi / sb_*_prove_multi call starts with, before any context is touched: the message of a
+// refusal is kept for the calling thread only (what sb_last_error(ctxs[0]) returns to it).
+static int multi_ctx_args(sb_ctx* const* ctxs, int n, const char* name) {
+    if (!ctxs || n < 1 || n > 64) return SB_ERR_ARG;
+    for (int i = 0; i < n; i++) if (!ctxs[i]) return SB_ERR_ARG;
+    for (int i = 0; i < n; i++)
+        for (int j = 0; j < i; j++)
+            if (ctxs[i] == ctxs[j]) {
+                t_err_ctx = ctxs[0];
+                t_err = std::string(name) + ": context " + std::to_string(i) + " is context " + std::to_string(j) + " again";
+                return SB_ERR_ARG;
+            }
+    return 0;
+}
+
+static int load_multi(sb_ctx* const* ctxs, int n, uint64_t* handles, const std::function<int(sb_ctx*, int, uint64_t, uint64_t*)>& load,
+                      int (*release)(sb_ctx*, uint64_t), const char* name) {
+    if (int rc = multi_ctx_args(ctxs, n, name)) return rc;
+    if (!handles) return fail(ctxs[0], SB_ERR_ARG, "null argument");
+    for (int i = 0; i < n; i++) handles[i] = 0;
+    const uint64_t id = ++g_multi_loads;
+    std::vector<std::future<int>> f;
+    for (int i = 0; i < n; i++)
+        f.push_back(std::async(std::launch::async, [&, i]() {
+            sb_ctx* c = ctxs[i];
+            SB_LOCK(c);
+            cudaSetDevice(c->device);
+            int rc = load(c, i, n > 1 ? id : 0, &handles[i]);
+            const int d0 = ctxs[0]->device;
+            int can = 0;
+            if (!rc && c->device != d0 && cudaDeviceCanAccessPeer(&can, c->device, d0) == cudaSuccess && can) {
+                cudaError_t e = cudaDeviceEnablePeerAccess(d0, 0);
+                if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) rc = cuda_fail(c, e, "cudaDeviceEnablePeerAccess");
+                cudaGetLastError();
+            }
+            return rc;
+        }));
+    std::vector<int> rcs(n);
+    for (int i = 0; i < n; i++) rcs[i] = f[i].get();
+    for (int i = 0; i < n; i++) {
+        if (!rcs[i]) continue;
+        const std::string msg = ctxs[i]->err;
+        for (int j = 0; j < n; j++) if (handles[j]) { release(ctxs[j], handles[j]); handles[j] = 0; }
+        return fail(ctxs[0], rcs[i], msg);
+    }
+    return 0;
+}
+
+// Argument checks of sb_*_prove_multi, before any device work: pointers, n, distinct contexts of one curve.  Then every
+// context is locked (in address order, so that calls on overlapping sets of contexts cannot deadlock) and the handles
+// are checked: keys[i] = rank i of one multi load (n = 1: a single-device key).
+template <class K> static int prove_multi_args(sb_ctx* const* ctxs, const uint64_t* handles, int n, const void* witness, const void* blinders,
+                                               const void* proof, K* (*get)(sb_ctx*, uint64_t), const char* name,
+                                               std::vector<std::unique_lock<std::recursive_mutex>>& locks, std::vector<K*>& keys) {
+    if (int rc = multi_ctx_args(ctxs, n, name)) return rc;
+    sb_ctx* c0 = ctxs[0];
+    if (!handles || !witness || !blinders || !proof) return fail(c0, SB_ERR_ARG, "null argument");
+    for (int i = 0; i < n; i++)
+        if (ctxs[i]->curve != c0->curve) return fail(c0, SB_ERR_ARG, std::string(name) + ": the contexts are not all of one curve");
+    std::vector<sb_ctx*> order(ctxs, ctxs + n);
+    std::sort(order.begin(), order.end(), std::less<sb_ctx*>());
+    for (sb_ctx* c : order) locks.emplace_back(c->mu);
+    keys.assign(n, nullptr);
+    for (int i = 0; i < n; i++) {
+        keys[i] = get(ctxs[i], handles[i]);
+        if (!keys[i]) return fail(c0, SB_ERR_ARG, std::string(name) + ": invalid handle of rank " + std::to_string(i));
+    }
+    for (int i = 0; i < n; i++) {
+        const K* k = keys[i];
+        const bool ok = n == 1 ? k->multi_id == 0 : (k->multi_id && k->multi_id == keys[0]->multi_id && k->rank == i && k->n_ranks == n);
+        if (!ok) return fail(c0, SB_ERR_ARG, std::string(name) + ": the handles do not come from one load_multi call of these " + std::to_string(n) + " contexts, in this order");
+    }
+    return 0;
+}
+
 extern "C" {
 
 int sb_plonk_load(sb_ctx* c, const uint8_t* zkey, uint64_t len, uint64_t* handle) { SB_LOCK(c);
@@ -1823,6 +1907,7 @@ int sb_plonk_info(sb_ctx* c, uint64_t h, uint32_t* n_vars, uint32_t* n_public, u
 uint32_t sb_plonk_proof_bytes(sb_ctx* c) { return c ? 9 * c->g1.aff_bytes + 6 * 32 : 0; }
 int sb_plonk_prove(sb_ctx* c, uint64_t h, const uint8_t* witness, uint64_t n_witness, const uint8_t* blinders, uint8_t* proof) { SB_LOCK(c);
     PlonkKeyDev* k = get_plonk_key(c, h); if (!k) return fail(c, SB_ERR_ARG, "invalid plonk handle");
+    if (k->multi_id) return fail(c, SB_ERR_ARG, MULTI_HANDLE(plonk));
     if (!witness || !blinders || !proof) return fail(c, SB_ERR_ARG, "null argument");
     cudaSetDevice(c->device);
     return c->curve == SB_BN254 ? plonk_prove_impl<BnFq, BnFr>(c, k, witness, n_witness, blinders, proof)
@@ -1830,6 +1915,7 @@ int sb_plonk_prove(sb_ctx* c, uint64_t h, const uint8_t* witness, uint64_t n_wit
 }
 int sb_plonk_prove_resident(sb_ctx* c, uint64_t h, const uint8_t* blinders, uint8_t* proof) { SB_LOCK(c);
     PlonkKeyDev* k = get_plonk_key(c, h); if (!k) return fail(c, SB_ERR_ARG, "invalid plonk handle");
+    if (k->multi_id) return fail(c, SB_ERR_ARG, MULTI_HANDLE(plonk));
     if (!blinders || !proof) return fail(c, SB_ERR_ARG, "null argument");
     if (!k->n_wit_resident) return fail(c, SB_ERR_ARG, "no witness resident for this proving key: call sb_plonk_prove first");
     cudaSetDevice(c->device);
@@ -1839,6 +1925,7 @@ int sb_plonk_prove_resident(sb_ctx* c, uint64_t h, const uint8_t* blinders, uint
 int sb_plonk_prove_batch(sb_ctx* c, uint64_t h, const uint8_t* witnesses, uint64_t n_witness, uint32_t count, const uint8_t* blinders,
                          uint8_t* proofs, int32_t* status) { SB_LOCK(c);
     PlonkKeyDev* k = get_plonk_key(c, h); if (!k) return fail(c, SB_ERR_ARG, "invalid plonk handle");
+    if (k->multi_id) return fail(c, SB_ERR_ARG, MULTI_HANDLE(plonk));
     if (n_witness != (uint64_t)k->z.nVars - k->z.nAdditions)                                          // plonk_prove.js:66-68
         return fail(c, SB_ERR_ARG, "Invalid witness length. Circuit: " + std::to_string(k->z.nVars) + ", witness: " + std::to_string(n_witness) + ", " + std::to_string(k->z.nAdditions));
     if (count == 0) return SB_OK;
@@ -1871,12 +1958,14 @@ int sb_fflonk_info(sb_ctx* c, uint64_t h, uint32_t* n_vars, uint32_t* n_public, 
 uint32_t sb_fflonk_proof_bytes(sb_ctx* c) { return c ? 4 * c->g1.aff_bytes + 16 * 32 : 0; }
 int sb_fflonk_prove(sb_ctx* c, uint64_t h, const uint8_t* witness, uint64_t n_witness, const uint8_t* blinders, uint8_t* proof) { SB_LOCK(c);
     FflonkKeyDev* k = get_fflonk_key(c, h); if (!k) return fail(c, SB_ERR_ARG, "invalid fflonk handle");
+    if (k->multi_id) return fail(c, SB_ERR_ARG, MULTI_HANDLE(fflonk));
     if (!witness || !blinders || !proof) return fail(c, SB_ERR_ARG, "null argument");
     cudaSetDevice(c->device);
     return fflonk_prove_impl<BnFq, BnFr>(c, k, witness, n_witness, blinders, proof);
 }
 int sb_fflonk_prove_resident(sb_ctx* c, uint64_t h, const uint8_t* blinders, uint8_t* proof) { SB_LOCK(c);
     FflonkKeyDev* k = get_fflonk_key(c, h); if (!k) return fail(c, SB_ERR_ARG, "invalid fflonk handle");
+    if (k->multi_id) return fail(c, SB_ERR_ARG, MULTI_HANDLE(fflonk));
     if (!blinders || !proof) return fail(c, SB_ERR_ARG, "null argument");
     if (!k->n_wit_resident) return fail(c, SB_ERR_ARG, "no witness resident for this proving key: call sb_fflonk_prove first");
     cudaSetDevice(c->device);
@@ -1885,6 +1974,7 @@ int sb_fflonk_prove_resident(sb_ctx* c, uint64_t h, const uint8_t* blinders, uin
 int sb_fflonk_prove_batch(sb_ctx* c, uint64_t h, const uint8_t* witnesses, uint64_t n_witness, uint32_t count, const uint8_t* blinders,
                           uint8_t* proofs, int32_t* status) { SB_LOCK(c);
     FflonkKeyDev* k = get_fflonk_key(c, h); if (!k) return fail(c, SB_ERR_ARG, "invalid fflonk handle");
+    if (k->multi_id) return fail(c, SB_ERR_ARG, MULTI_HANDLE(fflonk));
     if (n_witness != (uint64_t)k->z.nVars - k->z.nAdditions)                                          // fflonk_prove.js:79-81
         return fail(c, SB_ERR_ARG, "Invalid witness length. Circuit: " + std::to_string(k->z.nVars) + ", witness: " + std::to_string(n_witness) + ", " + std::to_string(k->z.nAdditions));
     if (count == 0) return SB_OK;
@@ -1897,6 +1987,53 @@ int sb_fflonk_release(sb_ctx* c, uint64_t h) { SB_LOCK(c);
     cudaSetDevice(c->device); cudaStreamSynchronize(c->stream);
     fflonk_free_key(k); c->fflonk_keys[h - 1] = nullptr;
     return 0;
+}
+
+int sb_plonk_load_multi(sb_ctx* const* ctxs, int n, const uint8_t* zkey, uint64_t zkey_len, uint64_t* handles) {
+    if (!zkey) return SB_ERR_ARG;
+    return load_multi(ctxs, n, handles, [=](sb_ctx* c, int i, uint64_t id, uint64_t* h) {
+        return c->curve == SB_BN254 ? plonk_load_impl<BnFr>(c, zkey, zkey_len, h, i, id ? n : 1, id)
+                                    : plonk_load_impl<BlsFr>(c, zkey, zkey_len, h, i, id ? n : 1, id);
+    }, sb_plonk_release, "sb_plonk_load_multi");
+}
+int sb_plonk_prove_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, const uint8_t* witness, uint64_t n_witness,
+                         const uint8_t* blinders, uint8_t* proof) {
+    std::vector<std::unique_lock<std::recursive_mutex>> locks; std::vector<PlonkKeyDev*> keys;
+    int rc = prove_multi_args(ctxs, handles, n, witness, blinders, proof, get_plonk_key, "sb_plonk_prove_multi", locks, keys);
+    if (rc) return rc;
+    sb_ctx* c = ctxs[0];
+    if (n == 1) return sb_plonk_prove(c, handles[0], witness, n_witness, blinders, proof);
+    cudaSetDevice(c->device);
+    PlonkRanks rk{ctxs, (PlonkKeyBase* const*)nullptr, n, nullptr};
+    std::vector<PlonkKeyBase*> base(keys.begin(), keys.end()); rk.keys = base.data();
+    CU(c, cudaEventCreateWithFlags(&rk.ready, cudaEventDisableTiming));
+    if (c->curve == SB_BN254) { CudaShardedBackend<Fp<BnFr>, CudaPlonkBackend> be; be.ranks = &rk; rc = plonk_prove_impl<BnFq, BnFr>(c, keys[0], witness, n_witness, blinders, proof, be); }
+    else { CudaShardedBackend<Fp<BlsFr>, CudaPlonkBackend> be; be.ranks = &rk; rc = plonk_prove_impl<BlsFq, BlsFr>(c, keys[0], witness, n_witness, blinders, proof, be); }
+    cudaEventDestroy(rk.ready);
+    return rc;
+}
+int sb_fflonk_load_multi(sb_ctx* const* ctxs, int n, const uint8_t* zkey, uint64_t zkey_len, uint64_t* handles) {
+    if (!zkey) return SB_ERR_ARG;
+    return load_multi(ctxs, n, handles, [=](sb_ctx* c, int i, uint64_t id, uint64_t* h) {
+        if (c->curve != SB_BN254) return fail(c, SB_ERR_ARG, "fflonk is defined on bn128 only (src/fflonk_setup.js:534-557)");
+        return fflonk_load_impl<BnFr>(c, zkey, zkey_len, h, i, id ? n : 1, id);
+    }, sb_fflonk_release, "sb_fflonk_load_multi");
+}
+int sb_fflonk_prove_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, const uint8_t* witness, uint64_t n_witness,
+                          const uint8_t* blinders, uint8_t* proof) {
+    std::vector<std::unique_lock<std::recursive_mutex>> locks; std::vector<FflonkKeyDev*> keys;
+    int rc = prove_multi_args(ctxs, handles, n, witness, blinders, proof, get_fflonk_key, "sb_fflonk_prove_multi", locks, keys);
+    if (rc) return rc;
+    sb_ctx* c = ctxs[0];
+    if (n == 1) return sb_fflonk_prove(c, handles[0], witness, n_witness, blinders, proof);
+    cudaSetDevice(c->device);
+    PlonkRanks rk{ctxs, (PlonkKeyBase* const*)nullptr, n, nullptr};
+    std::vector<PlonkKeyBase*> base(keys.begin(), keys.end()); rk.keys = base.data();
+    CU(c, cudaEventCreateWithFlags(&rk.ready, cudaEventDisableTiming));
+    CudaShardedBackend<Fp<BnFr>, CudaFflonkBackend> be; be.ranks = &rk;
+    rc = fflonk_prove_impl<BnFq, BnFr>(c, keys[0], witness, n_witness, blinders, proof, be);
+    cudaEventDestroy(rk.ready);
+    return rc;
 }
 
 }  // extern "C"

@@ -13,6 +13,7 @@ import numpy as np
 
 from .curve import Curve, SbError, _arr, _ptr, getCurveFromQ
 from .groth16 import _from_mont, random_fr, read_binfile, read_wtns_header
+from .plonk import ShardedProvingKey as _PlonkSharded
 
 POINTS = ("C1", "C2", "W1", "W2")
 EVALS = ("ql", "qr", "qm", "qo", "qc", "s1", "s2", "s3", "a", "b", "c", "z", "zw", "t1w", "t2w", "inv")
@@ -124,6 +125,16 @@ class ProvingKey:
             self.handle = 0
         if self._own_curve:
             self.curve.terminate()
+
+
+class ShardedProvingKey(_PlonkSharded):
+    """An fflonk zkey spread over several contexts so that one proof uses all of them (sb_fflonk_load_multi /
+    sb_fflonk_prove_multi), with the interface of plonk.ShardedProvingKey: curves[0] is rank 0, every context holds a
+    range of the 9n + 18 PTau points and its part of each commitment; curves may also be device indices."""
+
+    PROTO, N_BLINDERS = "fflonk", 9
+    read_header = staticmethod(read_zkey_header_fflonk)
+    to_object = staticmethod(proof_to_object)
 
 
 def prove(zkey, wtns: bytes, blinders: bytes | None = None, logger=None, options=None):

@@ -129,6 +129,80 @@ class ProvingKey:
             self.curve.terminate()
 
 
+class ShardedProvingKey:
+    """A PLONK zkey spread over several contexts so that one proof uses all of them (sb_plonk_load_multi /
+    sb_plonk_prove_multi).  curves[0] is rank 0: it holds the key and runs the proof; every context holds a contiguous
+    range of the PTau points and computes that part of each commitment.  curves are Curve objects of the key's curve
+    (several may be on one device) or device indices, for which the key makes its own Curve and closes it on release().
+    Proofs are byte-identical to ProvingKey.prove_raw with the same witness and blinders."""
+
+    PROTO, N_BLINDERS = "plonk", 11
+    read_header = staticmethod(read_zkey_header_plonk)
+    to_object = staticmethod(proof_to_object)
+
+    def __init__(self, zkey: bytes, curves):
+        zkey = bytes(zkey)
+        self.header = self.read_header(zkey)
+        if not curves:
+            raise SbError("at least one curve is needed")
+        self.curves, self._own, self.handles = [], [], None
+        try:
+            for c in curves:
+                if isinstance(c, int):
+                    c = getCurveFromQ(self.header["q"], c)
+                    self._own.append(c)
+                self.curves.append(c)
+            n = len(self.curves)
+            self._ctxs = (ctypes.c_void_p * n)(*[c.handle.value for c in self.curves])
+            handles = (ctypes.c_uint64 * n)()
+            buf = np.frombuffer(zkey, np.uint8)
+            c0 = self.curves[0]
+            c0.check(getattr(c0.lib, f"sb_{self.PROTO}_load_multi")(self._ctxs, n, _ptr(buf), buf.size, handles))
+            self.handles = handles
+        except BaseException:
+            self.release()
+            raise
+        for k in ("nVars", "nPublic", "domainSize", "nAdditions"):
+            setattr(self, k, self.header[k])
+
+    @property
+    def curve(self):
+        return self.curves[0]
+
+    def prove_raw(self, witness, blinders: bytes) -> bytes:
+        """witness = wtns section 2 ((nVars - nAdditions) x 32 bytes, plain LE); blinders = N_BLINDERS x 32 Montgomery bytes."""
+        if len(blinders) != self.N_BLINDERS * 32:
+            raise SbError(f"blinders must be {self.N_BLINDERS} field elements")
+        if witness is None:
+            raise SbError("a sharded key proves from a host witness only")
+        c = self.curves[0]
+        out = np.empty(getattr(c.lib, f"sb_{self.PROTO}_proof_bytes")(c.handle), np.uint8)
+        w = _arr(witness)
+        c.check(getattr(c.lib, f"sb_{self.PROTO}_prove_multi")(self._ctxs, self.handles, len(self.curves), _ptr(w), w.size // 32,
+                                                                bytes(blinders), _ptr(out)))
+        return out.tobytes()
+
+    def prove(self, wtns: bytes, blinders: bytes | None = None):
+        """(proof, publicSignals) as the module's prove."""
+        wh, W = read_wtns_header(bytes(wtns))
+        if wh["q"] != self.header["r"]:
+            raise SbError("Curve of the witness does not match the curve of the proving key")
+        if blinders is None:
+            blinders = b"".join(random_fr(self.curve) for _ in range(self.N_BLINDERS))
+        raw = self.prove_raw(np.frombuffer(W, np.uint8), blinders)
+        pub = [str(int.from_bytes(W[i * 32:(i + 1) * 32], "little")) for i in range(1, self.nPublic + 1)]
+        return self.to_object(self.curve, raw), pub
+
+    def release(self):
+        if self.handles is not None:
+            for c, h in zip(self.curves, self.handles):
+                getattr(c.lib, f"sb_{self.PROTO}_release")(c.handle, h)
+            self.handles = None
+        for c in self._own:
+            c.terminate()
+        self._own = []
+
+
 def prove(zkey, wtns: bytes, blinders: bytes | None = None, logger=None, options=None):
     """plonk16Prove(zkeyFileName, witnessFileName) -> (proof, publicSignals); zkey may be bytes or a ProvingKey."""
     pk = zkey if isinstance(zkey, ProvingKey) else ProvingKey(zkey)
