@@ -294,7 +294,7 @@ double sb_calibrate(sb_ctx* ctx, int what);
  *   2  1 = run every stream of a prove call serialised on one stream (per-kernel-class timing, sb_last_stat 8..15)
  *   3  1 = ignore the precomputed window tables (plain windowed Pippenger on the raw bases)
  *   6  log2 of the points per MSM chunk (test hook; 0 = default)
- *   7  log2 of the largest NTT tile (10..12)
+ *   7  log2 of the largest NTT tile (10..12; default 11, the value to restore: 0 is refused)
  *   8  0 = no pinned staging of pageable host buffers
  *  13  MSM window bits c, 3..22 (test hook; 0 = default: chosen from the number of points).  Applies wherever a geometry
  *      is chosen: per chunk for MSMs on unregistered bases, and for window tables when they are built, i.e. when bases are
@@ -325,6 +325,16 @@ int sb_generator(sb_ctx* ctx, int group, uint8_t* out_affine);
  *    6  0-3     a, b -> a*b (2N limbs)            14  4-5   x -> x^2*R^-1      15  4-5   x -> R^2*x^-1, 0 -> 0
  * Operands other than to_mont / from_mont inputs must be below p.  Any other (field, op) pair is SB_ERR_ARG. */
 int sb_field_eval(sb_ctx* ctx, int field, int op, const uint8_t* in, uint64_t n, uint8_t* out);
+/* test hook: `count` Fr transforms of n = 2^L elements of the context's curve through the launches the provers use:
+ * layout 0 runs fr_ntt_batch (count 1..4, each transform and its scratch at its own device offset, as Groth16's A, B, C),
+ * layout 1 runs fr_ntt_strided (count 1..65535 transforms back to back, as a batch of proofs).  inverse selects the
+ * twiddle table and does not scale; pre_first / pre_inc (both or neither) = the pre-multiplier first * inc^i by input
+ * position i on the first pass; post_scale = optional factor on the last pass.  Host in / out, count * n * 32 bytes,
+ * Montgomery, transform k at k * n * 32.  Every part of the device region is followed by a guard of sentinel bytes; a
+ * launch that writes into one fails the call with SB_ERR_CUDA.  L outside 0..Fr.s, count outside the layout's range, a
+ * layout other than 0 or 1, a null buffer or half a pre-multiplier is SB_ERR_ARG. */
+int sb_ntt_eval(sb_ctx* ctx, int L, int count, int layout, int inverse, const uint8_t* pre_first, const uint8_t* pre_inc,
+                const uint8_t* post_scale, const uint8_t* in, uint8_t* out);
 int sb_sync(sb_ctx* ctx);
 
 #ifdef __cplusplus

@@ -77,6 +77,7 @@ _SIGNATURES = {
     "sb_gen_points": (ctypes.c_int, [vp, ctypes.c_int, u64, u64, vp]),
     "sb_generator": (ctypes.c_int, [vp, ctypes.c_int, vp]),
     "sb_field_eval": (ctypes.c_int, [vp, ctypes.c_int, ctypes.c_int, vp, u64, vp]),
+    "sb_ntt_eval": (ctypes.c_int, [vp, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, vp, vp, vp, vp, vp]),
     "sb_groth16_prove_shard": (ctypes.c_int, [vp, u64, vp, u64, ctypes.c_int, ctypes.c_int, vp]),
     "sb_groth16_partials_bytes": (u32, [vp]),
     "sb_groth16_finish": (ctypes.c_int, [vp, u64, vp, ctypes.c_int, vp, vp, vp]),

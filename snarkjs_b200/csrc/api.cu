@@ -958,6 +958,53 @@ int sb_field_eval(sb_ctx* c, int field, int op, const uint8_t* in, uint64_t n, u
     CU(c, d2h(c, out, d_out, n * wo * 4));
     return 0;
 }
+// The NTT launches the provers make, on host data.  One device region holds the post-scale, then each input and scratch area
+// (per transform in layout 0, one for all in layout 1) with a guard of NTT_EVAL_GUARD sentinel elements after every part, so
+// that a launch reading another slot's data corrupts a neighbour instead of landing on the right bytes by chance, and a write
+// outside the areas is reported.
+static constexpr uint64_t NTT_EVAL_GUARD = 61;
+int sb_ntt_eval(sb_ctx* c, int L, int count, int layout, int inverse, const uint8_t* pre_first, const uint8_t* pre_inc,
+                const uint8_t* post_scale, const uint8_t* in, uint8_t* out) { SB_LOCK(c);
+    if (!c) return SB_ERR_ARG;
+    if (L < 0 || L > c->fr_s) return fail(c, SB_ERR_ARG, "sb_ntt_eval: L must be in 0..Fr.s");
+    if (layout != 0 && layout != 1) return fail(c, SB_ERR_ARG, "sb_ntt_eval: layout must be 0 (by pointer) or 1 (strided)");
+    if (count < 1 || count > (layout ? 65535 : 4)) return fail(c, SB_ERR_ARG, "sb_ntt_eval: count must be in 1..4 (layout 0) or 1..65535 (layout 1)");
+    if (!in || !out || !pre_first != !pre_inc) return fail(c, SB_ERR_ARG, "sb_ntt_eval: null argument");
+    cudaSetDevice(c->device);
+    const uint64_t n = 1ull << L, G = NTT_EVAL_GUARD;
+    const uint64_t span = layout ? (uint64_t)count * n : n;   // elements of one input or scratch area
+    const int areas = layout ? 1 : count;
+    const uint64_t total = 1 + G + 2 * (uint64_t)areas * (span + G);
+    uint8_t* d = (uint8_t*)c->io[0].get(total * 32);
+    if (!d) return fail(c, SB_ERR_NOMEM, "out of device memory");
+    auto area = [&](int k, int scratch) { return d + (1 + G + (2 * (uint64_t)k + scratch) * (span + G)) * 32; };
+    CU(c, cudaMemsetAsync(d, 0xA5, total * 32, c->stream));
+    for (int k = 0; k < areas; k++) CU(c, h2d(c, area(k, 0), in + (uint64_t)k * span * 32, span * 32));
+    if (post_scale) CU(c, cudaMemcpyAsync(d, post_scale, 32, cudaMemcpyHostToDevice, c->stream));
+    FrNttTables tb;
+    int rc = get_ntt_tab(c, L, inverse != 0, &tb); if (rc) return rc;
+    FrPre pre;
+    if (pre_first) { rc = get_pre(c, n, pre_first, pre_inc, &pre); if (rc) return rc; }
+    int side = 0, launches = 0;
+    if (layout == 0) {
+        void* a[4]; void* b[4];
+        for (int k = 0; k < 4; k++) { a[k] = area(k < count ? k : 0, 0); b[k] = area(k < count ? k : 0, 1); }
+        rc = fr_ntt_batch(c->curve, a, b, count, L, &tb, pre_first ? &pre : nullptr, post_scale ? d : nullptr, c->stream, &side, &launches);
+    } else {
+        rc = fr_ntt_strided(c->curve, area(0, 0), area(0, 1), count, L, &tb, pre_first ? &pre : nullptr, post_scale ? d : nullptr, c->stream, &side, &launches);
+    }
+    c->launches += launches;
+    if (rc) return cuda_fail(c, (cudaError_t)rc, layout ? "fr_ntt_strided" : "fr_ntt_batch");
+    std::vector<uint8_t> h(total * 32);
+    CU(c, d2h(c, h.data(), d, total * 32));
+    for (int k = 0; k <= 2 * areas; k++) {   // the guard after the post-scale slot and after every area
+        const uint8_t* g = h.data() + (k ? (1 + G + (uint64_t)k * (span + G) - G) : 1) * 32;
+        for (uint64_t i = 0; i < G * 32; i++)
+            if (g[i] != 0xA5) return fail(c, SB_ERR_CUDA, "sb_ntt_eval: a launch wrote outside its transforms");
+    }
+    for (int k = 0; k < areas; k++) memcpy(out + (uint64_t)k * span * 32, h.data() + (area(k, side) - d), span * 32);
+    return 0;
+}
 int sb_generator(sb_ctx* c, int group, uint8_t* out) { SB_LOCK(c);
     if (!c || (group != SB_G1 && group != SB_G2)) return SB_ERR_ARG;
     const std::vector<uint8_t>& g = group == SB_G1 ? c->gen1 : c->gen2;

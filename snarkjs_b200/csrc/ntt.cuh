@@ -160,7 +160,7 @@ k_ntt_pass(NttBatch<F> io, int L, int lgp, int deg, int logc,
         uint32_t col, b; uint64_t dst;
         if (lgp == 0) { b = e & (r - 1); col = e >> deg; dst = ((idx0 + col) << deg) + b; }
         else { col = e & (C - 1); b = e >> logc; uint64_t index = idx0 + col, k = index & pmask; dst = ((index - k) << deg) + k + ((uint64_t)b << lgp); }
-        uint32_t rb = __brev(b) >> (32 - deg);
+        uint32_t rb = deg ? __brev(b) >> (32 - deg) : 0;                   // deg = 0: the one-element transform of n = 1
         F x = lds_fe<F>(slo, shi, pos(rb, col));
         if (post_scale) x = F::mul(x, sc);
         stg_fe<F>(out + dst, x);
@@ -223,7 +223,8 @@ struct NttPlan { int npass; int deg[8]; int logc[8]; };
 extern int g_ntt_tile_log;   // log2 of the largest tile (elements); 12 = 128 KiB smem (1 CTA/SM), 11 = 64 KiB (3 CTAs/SM)
 inline NttPlan ntt_plan(int L) {
     NttPlan pl{};
-    if (L <= NTT_DMAX) { pl.npass = 1; pl.deg[0] = L; pl.logc[0] = 0; if (L == 0) pl.npass = 0; return pl; }
+    // n = 1 still takes one (degree-0) pass: it applies the pre-multiplier and the post-scale
+    if (L <= NTT_DMAX) { pl.npass = 1; pl.deg[0] = L; pl.logc[0] = 0; return pl; }
     int np = (L + NTT_DMAX - 1) / NTT_DMAX;
     int base = L / np, rem = L % np;
     pl.npass = np;
