@@ -323,6 +323,13 @@ int sb_generator(sb_ctx* ctx, int group, uint8_t* out_affine);
  *    5  0-2     x, y, u, v -> (x*y + u*v)*R^-1    12  4-5   x, y -> x*y*R^-1 (dual-product schoolbook)
  *               (mul2: not on BLS12-381 Fr)       13  4-5   x, y -> x*y*R^-1 (lazy Karatsuba)
  *    6  0-3     a, b -> a*b (2N limbs)            14  4-5   x -> x^2*R^-1      15  4-5   x -> R^2*x^-1, 0 -> 0
+ *   Point ops (csrc/ec.cuh, a = 0 curves) name the group by its base field: 0 BN254 G1, 2 BLS12-381 G1, 4 BN254 G2,
+ *   5 BLS12-381 G2.  Coordinates are Montgomery elements of that field; an affine point is x, y, an XYZZ point
+ *   x, y, zz, zzz (x = X/ZZ, y = Y/ZZZ, infinity: zz = 0; the results write infinity as all zeros).
+ *   16  0,2,4,5  acc (XYZZ), q (affine) -> acc.add_affine(q)   q must not be infinity, (0, 0): the MSM drops such bases
+ *   17  0,2,4,5  acc, q (XYZZ) -> acc.add_i(q)                 (the inlined addition of the MSM reduction kernels)
+ *   18  0,2,4,5  acc, q (XYZZ) -> acc.add(q)
+ *   19  0,2,4,5  p (XYZZ) -> dbl(p)                 20  0,2,4,5  p (affine) -> dbl_affine(p)
  * Operands other than to_mont / from_mont inputs must be below p.  Any other (field, op) pair is SB_ERR_ARG. */
 int sb_field_eval(sb_ctx* ctx, int field, int op, const uint8_t* in, uint64_t n, uint8_t* out);
 /* test hook: `count` Fr transforms of n = 2^L elements of the context's curve through the launches the provers use:

@@ -4,6 +4,8 @@
 //
 // Fields (the oracle's F_* ids, then the two Fq2): 0 BN254 Fq, 1 BN254 Fr, 2 BLS12-381 Fq, 3 BLS12-381 Fr, 4 BN254 Fq2,
 // 5 BLS12-381 Fq2.  A record is k little-endian elements of N 32-bit limbs (N of the base field); an Fq2 element is c0 || c1.
+// The point ops name a group by its base field: 0 BN254 G1, 2 BLS12-381 G1, 4 BN254 G2, 5 BLS12-381 G2; a point is its
+// coordinates in that order (x y for affine, x y zz zzz for XYZZ), each one element of the base field.
 #pragma once
 #include "ec.cuh"
 
@@ -22,6 +24,10 @@ enum {
     // Fq2 (fields 4-5)
     FE_FP2_MUL_I, FE_FP2_MUL_LAZY,                   // x y -> x*y: dual-product schoolbook, lazy Karatsuba
     FE_FP2_SQR_I, FE_FP2_INV,                        // x -> x^2, x -> x^-1 (0 -> 0)
+    // XYZZ points (fields 0, 2, 4, 5)
+    FE_EC_ADD_AFFINE,                                // acc q -> acc.add_affine(q) (acc XYZZ, q affine, not infinity)
+    FE_EC_ADD_I, FE_EC_ADD,                          // acc q -> acc.add_i(q), acc.add(q) (both XYZZ)
+    FE_EC_DBL, FE_EC_DBL_AFFINE,                     // p -> dbl(p) (XYZZ), p -> dbl_affine(p) (affine)
     FE_NOPS
 };
 
@@ -33,6 +39,16 @@ SB_CONSTEXPR_HD constexpr bool field_eval_has_mul2(int field) {
 SB_CONSTEXPR_HD constexpr int field_eval_words(int field, int op, bool out) {
     if (field < 0 || field >= FE_NFIELDS) return 0;
     const int n = (field == FE_BLS_FQ || field == FE_BLS_FQ2) ? 12 : 8;
+    if (op >= FE_EC_ADD_AFFINE && op < FE_NOPS) {
+        if (field == FE_BN_FR || field == FE_BLS_FR) return 0;
+        const int e = field >= FE_BN_FQ2 ? 2 * n : n;   // words per coordinate
+        switch (op) {
+        case FE_EC_ADD_AFFINE: return out ? 4 * e : 6 * e;
+        case FE_EC_ADD_I: case FE_EC_ADD: return out ? 4 * e : 8 * e;
+        case FE_EC_DBL: return 4 * e;
+        default: return out ? 4 * e : 2 * e;       // FE_EC_DBL_AFFINE
+        }
+    }
     if (field >= FE_BN_FQ2) {
         if (op == FE_FP2_MUL_I || op == FE_FP2_MUL_LAZY) return out ? 2 * n : 4 * n;
         if (op == FE_FP2_SQR_I || op == FE_FP2_INV) return 2 * n;
@@ -109,8 +125,51 @@ template <class P> SB_HD void field_eval_fp2(int op, const uint32_t* in, uint32_
     fe_st(out, r.a); fe_st(out + N, r.b);
 }
 
+// coordinates of an Fp or Fp2 point
+template <class P> SB_HD void ec_ld(Fp<P>& x, const uint32_t* w) { x = fe_ld<P>(w); }
+template <class P> SB_HD void ec_ld(Fp2<P>& x, const uint32_t* w) { x.a = fe_ld<P>(w); x.b = fe_ld<P>(w + P::N); }
+template <class P> SB_HD void ec_st(uint32_t* w, const Fp<P>& x) { fe_st(w, x); }
+template <class P> SB_HD void ec_st(uint32_t* w, const Fp2<P>& x) { fe_st(w, x.a); fe_st(w + P::N, x.b); }
+template <class F> SB_HD XYZZ<F> ec_ld_xyzz(const uint32_t* w) {
+    constexpr int E = sizeof(F) / 4;
+    XYZZ<F> p;
+    ec_ld(p.x, w); ec_ld(p.y, w + E); ec_ld(p.zz, w + 2 * E); ec_ld(p.zzz, w + 3 * E);
+    return p;
+}
+
+// The point formulas as the MSM and group FFT kernels call them.  add_affine is handed `one` = F::one() as k_accumulate
+// hands it; its q is never infinity there (k_accumulate drops (0, 0) bases before the addition), so no record may be.
+template <class F> SB_HD void field_eval_ec(int op, const uint32_t* in, uint32_t* out) {
+    constexpr int E = sizeof(F) / 4;                 // words per coordinate
+    static_assert(E * 4 == sizeof(F), "a coordinate is whole 32-bit words");
+    XYZZ<F> r;
+    F qx, qy;
+    switch (op) {
+    case FE_EC_ADD_AFFINE:
+        r = ec_ld_xyzz<F>(in); ec_ld(qx, in + 4 * E); ec_ld(qy, in + 5 * E);
+        r.add_affine(qx, qy, F::one());
+        break;
+    case FE_EC_ADD_I: r = ec_ld_xyzz<F>(in); r.add_i(ec_ld_xyzz<F>(in + 4 * E)); break;
+    case FE_EC_ADD: r = ec_ld_xyzz<F>(in); r.add(ec_ld_xyzz<F>(in + 4 * E)); break;
+    case FE_EC_DBL: r = XYZZ<F>::dbl(ec_ld_xyzz<F>(in)); break;
+    case FE_EC_DBL_AFFINE: ec_ld(qx, in); ec_ld(qy, in + E); r = XYZZ<F>::dbl_affine(qx, qy, F::one()); break;
+    default: return;
+    }
+    ec_st(out, r.x); ec_st(out + E, r.y); ec_st(out + 2 * E, r.zz); ec_st(out + 3 * E, r.zzz);
+}
+
 // one record of (field, op); the caller has checked field_eval_words(field, op, ...) != 0
 SB_HD void field_eval_record(int field, int op, const uint32_t* in, uint32_t* out) {
+    if (op >= FE_EC_ADD_AFFINE) {
+        switch (field) {
+        case FE_BN_FQ: field_eval_ec<Fp<BnFq>>(op, in, out); break;
+        case FE_BLS_FQ: field_eval_ec<Fp<BlsFq>>(op, in, out); break;
+        case FE_BN_FQ2: field_eval_ec<Fp2<BnFq>>(op, in, out); break;
+        case FE_BLS_FQ2: field_eval_ec<Fp2<BlsFq>>(op, in, out); break;
+        default: break;
+        }
+        return;
+    }
     switch (field) {
     case FE_BN_FQ: field_eval_fp<BnFq>(op, in, out); break;
     case FE_BN_FR: field_eval_fp<BnFr>(op, in, out); break;

@@ -39,6 +39,7 @@ FP_OPS = {"add": 0, "sub": 1, "neg": 2, "dbl": 3, "mul": 4, "mul2": 5, "mul_wide
           "from_mont": 9, "inv_binary": 10, "inv": 11}
 FP2_OPS = {"mul_i": 12, "mul_lazy": 13, "sqr_i": 14, "inv": 15}
 OP_NAMES = {**{v: k for k, v in FP_OPS.items()}, **{v: "fp2_" + k for k, v in FP2_OPS.items()}}
+FE_NOPS = 21                   # the first op sb_field_eval does not define; 16-20 are the point ops of tests/ec_edges.py
 N_RANDOM = 1000
 
 

@@ -6,6 +6,7 @@ import functools
 import numpy as np
 import pytest
 
+from tests import ec_edges as EC
 from tests import field_edges as FE
 
 pytestmark = pytest.mark.gpu
@@ -57,12 +58,16 @@ def test_field_primitive_edges(curves, field, op):
         pytest.fail(f"{len(bad)}+ mismatching records, first ones:\n" + "\n".join(bad))
 
 
-def test_field_eval_refuses_undefined_pairs(curves):
+def test_field_eval_refuses_undefined_field_op_pairs(curves):
+    """Ops past the last point op, point ops on the Fr fields and Fp ops on Fq2 are SB_ERR_ARG, as are unknown fields."""
     c = curves["bls12381"]
     buf = np.zeros(4 * 48, np.uint8)
     out = np.zeros(4 * 48, np.uint8)
-    for field, op in ((3, FE.FP_OPS["mul2"]), (0, FE.FP2_OPS["mul_i"]), (4, FE.FP_OPS["add"]), (5, FE.FP_OPS["mul"]),
-                      (6, 0), (-1, 0), (0, 16), (0, -1)):
+    refused = [(3, FE.FP_OPS["mul2"]), (0, FE.FP2_OPS["mul_i"]), (6, 0), (-1, 0), (0, FE.FE_NOPS), (4, FE.FE_NOPS),
+               (0, -1)]
+    refused += [(f, op) for f in (4, 5) for op in FE.FP_OPS.values()]           # Fp ops are not defined on Fq2
+    refused += [(f, op) for f in (1, 3) for op in EC.EC_OPS.values()]           # no group over Fr
+    for field, op in refused:
         assert c.lib.sb_field_eval(c.handle, field, op, _ptr(buf), 1, _ptr(out)) == -1, (field, op)
         assert b"not defined" in c.lib.sb_last_error(c.handle)
     assert c.lib.sb_field_eval(None, 0, 0, _ptr(buf), 1, _ptr(out)) == -1
