@@ -125,6 +125,25 @@ int sb_groth16_prove_resident(sb_ctx* ctx, uint64_t handle, const uint8_t r[32],
 int sb_groth16_prove_batch(sb_ctx* ctx, uint64_t handle, const uint8_t* witnesses, uint64_t n_witness, uint32_t count,
                            const uint8_t* r, const uint8_t* s, uint8_t* proofs_out);
 int sb_groth16_release(sb_ctx* ctx, uint64_t handle);
+/* groth16Verify (src/groth16_verify.js:26-87) for count proofs against one verification key.
+ * vk = alpha1 (G1) || beta2 (G2) || gamma2 (G2) || delta2 (G2) || IC[0..n_public] (G1): affine Montgomery, all-zero =
+ *   infinity, i.e. the zkey's header points and section 3; vk_len must be (14 + 2 (n_public + 1)) * n8q; a vk point off its
+ *   curve or a coordinate >= q: SB_ERR_ARG.
+ * publics = count * n_public * 32 bytes, plain LE; proofs = count * 8*n8q bytes laid out as sb_groth16_prove writes them
+ *   (a coordinate >= q counts as not on the curve).
+ * status_out[k]: 0 verifies, 1 "Invalid proof", 2 "Public inputs are not valid.", 3 "Proof commitments are not valid."
+ *   (checked in that reference order: 2, then 3, then 1).  As in the reference, points are checked to be on their curves
+ *   (infinity included) and not for subgroup membership.  The proofs run in sub-batches of at most 2^15 (fewer for many
+ *   public inputs; sb_set_tuning(14) caps them).  count == 0 writes nothing.  sb_last_ms(0) = the whole call. */
+int sb_groth16_verify_batch(sb_ctx* ctx, const uint8_t* vk, uint64_t vk_len, uint32_t n_public,
+                            const uint8_t* publics, const uint8_t* proofs, uint32_t count, int32_t* status_out);
+/* test hook, the device pairing (csrc/pairing.cuh) on the context's curve over n records: op 0 Fq12 mul (a, b), 1 Fq12 square,
+ * 2 cyclotomic square, 3 inverse, 4 Frobenius (a -> a^q, a^(q^2), a^(q^3): three outputs), 5 Miller loop of one (G1, G2)
+ * pair, 6 final exponentiation, 7 full pairing.  Tower elements are 12 Montgomery Fq coefficients in ffjavascript's order
+ * (Fq12 = Fq6[w]/(w^2 - v), Fq6 = Fq2[v]/(v^3 - xi)); a pair is G1 x, y || G2 x.c0, x.c1, y.c0, y.c1, affine Montgomery, all
+ * zero = infinity.  The final exponentiation raises to c (q^12 - 1)/r with c = 2x(6x^2 + 3x + 1) on BN254, 3 on BLS12-381.
+ * Other ops: SB_ERR_ARG. */
+int sb_pairing_eval(sb_ctx* ctx, int op, const uint8_t* in, uint64_t n, uint8_t* out);
 /* ---- PLONK (src/plonk_prove.js:47-889), next-tier path per SURVEY §8f rank 3 ----------------------------------
  * sb_plonk_load: a PLONK zkey (protocol id 2, sections 2-14: src/zkey_utils.js:261-299, src/plonk_constants.js) goes to
  *   HBM once: selector / sigma / Lagrange polynomials in coefficient and 4n-evaluation form, wire maps, additions, and the
@@ -300,7 +319,8 @@ double sb_calibrate(sb_ctx* ctx, int what);
  *      is chosen: per chunk for MSMs on unregistered bases, and for window tables when they are built, i.e. when bases are
  *      registered or a key is loaded; a table keeps the c in force at that moment.  Tables are still skipped when
  *      W * n >= 2^31.  A large c costs memory: a plain MSM allocates W * 2^(c-1) buckets.
- *  14  most proofs per sub-batch of sb_groth16_prove_batch, sb_plonk_prove_batch and sb_fflonk_prove_batch, and rows per sub-batch of
+ *  14  most proofs per sub-batch of sb_groth16_prove_batch, sb_plonk_prove_batch, sb_fflonk_prove_batch and
+ *      sb_groth16_verify_batch, and rows per sub-batch of
  *      sb_msm_registered_batch (test hook;
  *      0 = default: as many as the 32-bit bucket keys and free device memory allow)
  * The Python mirror applies SB_TUNE="key=value,..." from the environment when it loads the library. */

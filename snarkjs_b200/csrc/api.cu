@@ -1836,6 +1836,7 @@ int sb_groth16_prove_wtns(sb_ctx* c, uint64_t h, const uint8_t* w, uint64_t wlen
 // PLONK (src/plonk_prove.js) — templates live outside the extern "C" block
 #include "api_plonk.inl"
 #include "api_fflonk.inl"
+#include "api_verify.inl"
 
 // ---- one PLONK / fflonk proof on several devices (sb_plonk_load_multi .. sb_fflonk_prove_multi)
 // a key of a multi load holds one PTau range only, so the single-device entries refuse it

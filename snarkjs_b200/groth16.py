@@ -244,3 +244,153 @@ def prove_batch(zkey, wtns_list, rs=None):
     finally:
         if not isinstance(zkey, ProvingKey):
             pk.release()
+
+
+# ------------------------------------------------------------------ verification (src/groth16_verify.js:26-87)
+VERIFY_MESSAGES = {1: "Invalid proof", 2: "Public inputs are not valid.", 3: "Proof commitments are not valid."}
+
+
+def _curve_of(name: str):
+    """(n8q, q, r, snarkjs name) of a curve named as snarkjs names it."""
+    from .curve import _Q, _R
+    key = {"BN128": "bn128", "BN254": "bn128", "ALTBN128": "bn128", "BLS12381": "bls12381"}.get(
+        str(name).upper().replace("-", "").replace("_", ""), name)
+    if key not in _R:
+        raise SbError(f"Curve not supported: {name}")
+    n8q = 32 if key == "bn128" else 48
+    return n8q, _Q[(n8q,)], _R[key], key
+
+
+def verification_key(zkey) -> dict:
+    """zkey export verificationkey for a Groth16 key (src/zkey_export_verificationkey.js): the fields groth16Verify reads, as
+    decimal strings (G.toObject + stringifyBigInts).  vk_alphabeta_12 is not produced."""
+    data = bytes(zkey)
+    z = read_zkey_header_groth16(data)
+    n8, q = z["n8q"], z["q"]
+    name = "bn128" if n8 == 32 else "bls12381"
+    f = lambda b: str(_from_mont(b, q, n8))
+
+    def g1(p):
+        return ["0", "1", "0"] if p == bytes(2 * n8) else [f(p[:n8]), f(p[n8:]), "1"]
+
+    def g2(p):
+        if p == bytes(4 * n8):
+            return [["0", "0"], ["1", "0"], ["0", "0"]]
+        return [[f(p[:n8]), f(p[n8:2 * n8])], [f(p[2 * n8:3 * n8]), f(p[3 * n8:])], ["1", "0"]]
+
+    pos, _ = z["sections"][3]
+    ic = [g1(data[pos + i * 2 * n8:pos + (i + 1) * 2 * n8]) for i in range(z["nPublic"] + 1)]
+    return {"protocol": "groth16", "curve": name, "nPublic": z["nPublic"], "vk_alpha_1": g1(z["vk_alpha_1"]),
+            "vk_beta_2": g2(z["vk_beta_2"]), "vk_gamma_2": g2(z["vk_gamma_2"]), "vk_delta_2": g2(z["vk_delta_2"]), "IC": ic}
+
+
+def _f2_mul(a, b, q):
+    return ((a[0] * b[0] - a[1] * b[1]) % q, (a[0] * b[1] + a[1] * b[0]) % q)
+
+
+def _f2_inv(a, q):
+    n = pow((a[0] * a[0] + a[1] * a[1]) % q, -1, q)
+    return (a[0] * n % q, -a[1] * n % q)
+
+
+def point_bytes(obj, group: int, n8q: int, q: int) -> bytes:
+    """G.fromObject (build/snarkjs.js:13486-13495 over F.fromObject :13042-13046) then affine Montgomery bytes: the object is
+    Jacobian (x, y, z), every coordinate taken mod q; z = 0 is infinity (all-zero bytes), otherwise (x/z^2, y/z^3)."""
+    R = 1 << (8 * n8q)
+    enc = lambda v: (v * R % q).to_bytes(n8q, "little")
+    if group == 1:
+        x, y = int(obj[0]) % q, int(obj[1]) % q
+        z = int(obj[2]) % q if len(obj) > 2 else 1
+        if z == 0:
+            return bytes(2 * n8q)
+        zi = pow(z, -1, q)
+        z2 = zi * zi % q
+        return enc(x * z2 % q) + enc(y * z2 * zi % q)
+    x = (int(obj[0][0]) % q, int(obj[0][1]) % q)
+    y = (int(obj[1][0]) % q, int(obj[1][1]) % q)
+    z = (int(obj[2][0]) % q, int(obj[2][1]) % q) if len(obj) > 2 else (1, 0)
+    if z == (0, 0):
+        return bytes(4 * n8q)
+    zi = _f2_inv(z, q)
+    z2 = _f2_mul(zi, zi, q)
+    ax, ay = _f2_mul(x, z2, q), _f2_mul(y, _f2_mul(z2, zi, q), q)
+    return enc(ax[0]) + enc(ax[1]) + enc(ay[0]) + enc(ay[1])
+
+
+def vk_bytes(vk_verifier: dict) -> bytes:
+    """The verification key as sb_groth16_verify_batch takes it: alpha1 || beta2 || gamma2 || delta2 || IC[0..nPublic]."""
+    n8, q, _r, _name = _curve_of(vk_verifier["curve"])
+    ic = vk_verifier["IC"]
+    if len(ic) != int(vk_verifier["nPublic"]) + 1:
+        raise SbError(f"IC has {len(ic)} points, nPublic is {vk_verifier['nPublic']}")
+    return (point_bytes(vk_verifier["vk_alpha_1"], 1, n8, q) + b"".join(point_bytes(vk_verifier[k], 2, n8, q)
+            for k in ("vk_beta_2", "vk_gamma_2", "vk_delta_2")) + b"".join(point_bytes(p, 1, n8, q) for p in ic))
+
+
+def proof_bytes(proof: dict, n8q: int, q: int) -> bytes:
+    return point_bytes(proof["pi_a"], 1, n8q, q) + point_bytes(proof["pi_b"], 2, n8q, q) + point_bytes(proof["pi_c"], 1, n8q, q)
+
+
+def publics_bytes(public_signals, r: int):
+    """Plain LE 32-byte public signals, or None when one cannot be written in 32 bytes (then it is >= r: status 2)."""
+    vals = [int(s) for s in public_signals]
+    if any(v < 0 or v >= r for v in vals):
+        return None
+    return b"".join(v.to_bytes(32, "little") for v in vals)
+
+
+def verify_status(vk_verifier: dict, items, curve: Curve | None = None) -> list:
+    """sb_groth16_verify_batch over [(publicSignals, proof), ...]: one status per item (0 verifies, else the key of
+    VERIFY_MESSAGES).  A proof with a signal count other than nPublic gets 1, as the reference's pairing would give it."""
+    n8, q, r, name = _curve_of(vk_verifier["curve"])
+    n_public = int(vk_verifier["nPublic"])
+    vk = np.frombuffer(vk_bytes(vk_verifier), np.uint8)
+    status = [None] * len(items)
+    pubs, prfs, slots = [], [], []
+    for k, (signals, proof) in enumerate(items):
+        pb = publics_bytes(signals, r)
+        if pb is None:
+            status[k] = 2
+        elif len(signals) != n_public:
+            status[k] = 1
+        else:
+            pubs.append(pb)
+            prfs.append(proof_bytes(proof, n8, q))
+            slots.append(k)
+    own = curve is None
+    cv = curve or Curve(name)
+    try:
+        count = len(slots)
+        out = np.zeros(max(count, 1), np.int32)
+        pub = np.frombuffer(b"".join(pubs) or b"\0", np.uint8)
+        prf = np.frombuffer(b"".join(prfs) or b"\0", np.uint8)
+        cv.check(cv.lib.sb_groth16_verify_batch(cv.handle, _ptr(vk), vk.size, n_public, _ptr(pub), _ptr(prf), count,
+                                                out.ctypes.data_as(ctypes.c_void_p)))
+    finally:
+        if own:
+            cv.terminate()
+    for j, k in enumerate(slots):
+        status[k] = int(out[j])
+    return status
+
+
+def verify_batch(vk_verifier: dict, items, logger=None, curve: Curve | None = None) -> list:
+    """groth16Verify over many (publicSignals, proof) pairs against one verification key, in one device call -> [bool]."""
+    st = verify_status(vk_verifier, items, curve)
+    if logger:
+        for s in st:
+            if s:
+                logger.error(VERIFY_MESSAGES[s])
+    return [s == 0 for s in st]
+
+
+def verify(vk_verifier: dict, publicSignals, proof: dict, logger=None, curve: Curve | None = None) -> bool:
+    """groth16Verify(vk_verifier, publicSignals, proof, logger) (src/groth16_verify.js:26-87): True, or False with the
+    reference's log message."""
+    s = verify_status(vk_verifier, [(publicSignals, proof)], curve)[0]
+    if logger:
+        if s:
+            logger.error(VERIFY_MESSAGES[s])
+        else:
+            logger.info("OK!")
+    return s == 0
