@@ -312,7 +312,8 @@ double sb_calibrate(sb_ctx* ctx, int what);
  *      windows of more than 2^20 buckets)
  *   2  1 = run every stream of a prove call serialised on one stream (per-kernel-class timing, sb_last_stat 8..15)
  *   3  1 = ignore the precomputed window tables (plain windowed Pippenger on the raw bases)
- *   6  log2 of the points per MSM chunk (test hook; 0 = default)
+ *   6  log2 of the points per MSM chunk, 1..23 (test hook; 0 = default: 2^23, the largest chunk the sort and the batch
+ *      limits are sized for)
  *   7  log2 of the largest NTT tile (10..12; default 11, the value to restore: 0 is refused)
  *   8  0 = no pinned staging of pageable host buffers
  *  13  MSM window bits c, 3..22 (test hook; 0 = default: chosen from the number of points).  Applies wherever a geometry

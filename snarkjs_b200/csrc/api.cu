@@ -923,7 +923,7 @@ int sb_set_tuning(int key, int value) {
     case 1: if (value != 0 && value != 1) return SB_ERR_ARG; g_msm_force_reduce = value; return 0;   // bucket reduction
     case 2: g_serial_prove = value; return 0;                                                           // serialised prove call
     case 3: g_no_tables = value; return 0;                                                              // no window tables
-    case 6: g_msm_chunk_log = value; return 0;                                                          // MSM chunk size
+    case 6: if (value < 0 || value > 23) return SB_ERR_ARG; g_msm_chunk_log = value; return 0;         // MSM chunk size
     case 7: if (value < 10 || value > 12) return SB_ERR_ARG; g_ntt_tile_log = value; return 0;         // NTT tile size
     case 8: g_stage_enabled = value; return 0;                                                          // pinned staging of pageable buffers
     case 13: if (value != 0 && (value < 3 || value > 22)) return SB_ERR_ARG; g_msm_force_c = value; return 0;   // MSM window bits

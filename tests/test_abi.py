@@ -66,6 +66,19 @@ def test_shard_range_partitions():
             assert tot == total and nxt == total
 
 
+def test_msm_chunk_tuning_is_bounded():
+    """sb_set_tuning(6, v) sets chunks of 2^v points: 0 (the 2^23 default) and 1..23 are taken; a negative log, one past the
+    default and shift counts of 64 and more (undefined for the 64-bit chunk size) are SB_ERR_ARG.  No device is needed."""
+    L = N.lib()
+    try:
+        for v in (0, 1, 23):
+            assert L.sb_set_tuning(6, v) == 0, v
+        for v in (-1, 24, 64, 1 << 30):
+            assert L.sb_set_tuning(6, v) == -1, v
+    finally:
+        assert L.sb_set_tuning(6, 0) == 0
+
+
 def test_prover_entry_points_reject_null_context():
     """The PLONK / fflonk entry points return SB_ERR_ARG (-1) instead of touching a null context."""
     L = N.lib()

@@ -2,8 +2,8 @@
 oracle's where checked (and verifies where the key is structured).  Covered: the reference fixture, chain keys of 13 to
 2000 gates (2000: window-table commitments), an unstructured 2^14 key, every BN254 shape key of tests/r1cs_shapes.py
 (refused ones with the single path's text), a key whose C0 is not the interleave of its parts; every way of running
-(sub-batches of 1 and 3, no window tables, serialised); a witness the reference rejects in the middle of a batch; the
-resident witness of sb_fflonk_prove_resident; and launches that do not grow with K."""
+(sub-batches of 1 and 3, no window tables, serialised, MSM chunks shorter than a row); a witness the reference rejects in
+the middle of a batch; the resident witness of sb_fflonk_prove_resident; and launches that do not grow with K."""
 import contextlib
 import ctypes
 import functools
@@ -175,7 +175,21 @@ def test_prove_batch_objects(curve):
         pk.release()
 
 
-@pytest.mark.parametrize("mode", ["sub1", "sub3", "no_tables", "serial"])
+def log_n(pk):
+    """log2 of the key's domain size n, from sb_fflonk_info"""
+    lib, c = pk.curve.lib, pk.curve
+    nv, npub, ds, na = (ctypes.c_uint32() for _ in range(4))
+    assert lib.sb_fflonk_info(c.handle, pk.handle, ctypes.byref(nv), ctypes.byref(npub), ctypes.byref(ds), ctypes.byref(na)) == 0
+    return ds.value.bit_length() - 1
+
+
+# MSM chunks of 2^(log2(n) + offset) points, shorter than the batch's rows of 9n: the batch commits row by row, chunk by
+# chunk, instead of one sorted MSM over all rows.  A row of 9n is then exactly 9 chunks (n), 4.5 chunks (2n), or one whole
+# chunk and n points (8n, where C1's 8n is exactly one chunk).
+CHUNKED = {"chunked-n": 0, "chunked-2n": 1, "chunked-8n": 3}
+
+
+@pytest.mark.parametrize("mode", ["sub1", "sub3", "no_tables", "serial"] + list(CHUNKED))
 def test_every_way_of_running_gives_the_same_bytes(curve, mode):
     import snarkjs_b200
     zkey, wl, _ = synth_case("g2000")
@@ -184,15 +198,22 @@ def test_every_way_of_running_gives_the_same_bytes(curve, mode):
     pk = snarkjs_b200.fflonk.ProvingKey(zkey, curve)
     try:
         want = [pk.prove_raw(payload(x), b) for x, b in zip(ws, bls)]
+        if mode in CHUNKED:
+            chunk = [(6, log_n(pk) + CHUNKED[mode])]
+            with tuning(curve.lib, chunk):                                # a key loaded before the setting
+                assert pk.prove_batch_raw([payload(x) for x in ws], bls) == want
     finally:
         pk.release()
-    settings = {"sub1": [(14, 1)], "sub3": [(14, 3)], "no_tables": [(3, 1)], "serial": [(2, 1)]}[mode]
-    with tuning(curve.lib, settings):
-        pk = snarkjs_b200.fflonk.ProvingKey(zkey, curve)        # loaded under the setting: no window tables in no_tables
-        try:
-            assert pk.prove_batch_raw([payload(x) for x in ws], bls) == want
-        finally:
-            pk.release()
+    # chunked: also without window tables, which makes the commitments plain-mode MSMs past a chunk
+    runs = ([chunk, chunk + [(3, 1)]] if mode in CHUNKED else
+            [{"sub1": [(14, 1)], "sub3": [(14, 3)], "no_tables": [(3, 1)], "serial": [(2, 1)]}[mode]])
+    for settings in runs:
+        with tuning(curve.lib, settings):
+            pk = snarkjs_b200.fflonk.ProvingKey(zkey, curve)        # loaded under the setting: no window tables in no_tables
+            try:
+                assert pk.prove_batch_raw([payload(x) for x in ws], bls) == want, settings
+            finally:
+                pk.release()
 
 
 def test_errors_and_state(curve):

@@ -1,8 +1,8 @@
 """GPU: sb_plonk_prove_batch.  Every batch proof is byte-identical to prove_raw of the same witness and blinders, and the
 oracle's where checked (and verifies where the key is structured).  Covered: the reference fixture and circuit2, chain keys
 of 13 to 16000 gates (4090: window-table commitments; 16000: 2^14 on unstructured points), several public inputs, deep
-additions and BLS12-381; every way of running (sub-batches of 1 and 3, no window tables); a witness the reference rejects
-in the middle of a batch; the resident witness of sb_plonk_prove_resident; and launches that do not grow with K."""
+additions and BLS12-381; every way of running (sub-batches of 1 and 3, no window tables, MSM chunks shorter than a
+row); a witness the reference rejects in the middle of a batch; the resident witness of sb_plonk_prove_resident; and launches that do not grow with K."""
 import contextlib
 import ctypes
 import functools
@@ -141,26 +141,46 @@ def test_prove_batch_objects(curves):
         pk.release()
 
 
+def log_n(pk):
+    """log2 of the key's domain size n, from sb_plonk_info"""
+    lib, c = pk.curve.lib, pk.curve
+    nv, npub, ds, na = (ctypes.c_uint32() for _ in range(4))
+    assert lib.sb_plonk_info(c.handle, pk.handle, ctypes.byref(nv), ctypes.byref(npub), ctypes.byref(ds), ctypes.byref(na)) == 0
+    return ds.value.bit_length() - 1
+
+
+# MSM chunks of 2^(log2(n) + offset) points, shorter than the batch's rows of n + 6: the batch commits row by row, chunk by
+# chunk, instead of one sorted MSM over all rows.  n / 2 puts a row over three chunks, n over two (the last of 6 points);
+# either way the single path's T1 and T2 (n + 1 points) end one point into a chunk.
+CHUNKED = {"chunked-half": -1, "chunked-n": 0}
+
+
 @pytest.mark.parametrize("label", ["g1000", "g4090"])
-@pytest.mark.parametrize("mode", ["sub1", "sub3", "no_tables"])
+@pytest.mark.parametrize("mode", ["sub1", "sub3", "no_tables"] + list(CHUNKED))
 def test_every_way_of_running_gives_the_same_bytes(curves, label, mode):
     import snarkjs_b200
     zkey, wl, _ = synth_case(label)
     ws = list(wl[:7])
     bls = blinders(BN, 7)
+    lib = curves[BN].lib
     pk = snarkjs_b200.plonk.ProvingKey(zkey, curves[BN])
     try:
         want = [pk.prove_raw(payload(x), b) for x, b in zip(ws, bls)]
+        if mode in CHUNKED:
+            chunk = [(6, log_n(pk) + CHUNKED[mode])]
+            with tuning(lib, chunk):                                      # a key loaded before the setting
+                assert pk.prove_batch_raw([payload(x) for x in ws], bls) == want
     finally:
         pk.release()
-    lib = curves[BN].lib
-    settings = {"sub1": [(14, 1)], "sub3": [(14, 3)], "no_tables": [(3, 1)]}[mode]
-    with tuning(lib, settings):
-        pk = snarkjs_b200.plonk.ProvingKey(zkey, curves[BN])        # loaded under the setting: no window tables in no_tables
-        try:
-            assert pk.prove_batch_raw([payload(x) for x in ws], bls) == want
-        finally:
-            pk.release()
+    # chunked: also without window tables, which makes g4090's commitments plain-mode MSMs past a chunk
+    runs = [chunk, chunk + [(3, 1)]] if mode in CHUNKED else [{"sub1": [(14, 1)], "sub3": [(14, 3)], "no_tables": [(3, 1)]}[mode]]
+    for settings in runs:
+        with tuning(lib, settings):
+            pk = snarkjs_b200.plonk.ProvingKey(zkey, curves[BN])        # loaded under the setting: no window tables in no_tables
+            try:
+                assert pk.prove_batch_raw([payload(x) for x in ws], bls) == want, settings
+            finally:
+                pk.release()
 
 
 def test_errors_and_state(curves):

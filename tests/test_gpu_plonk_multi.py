@@ -3,8 +3,8 @@ commitment summed from one MSM partial per rank over its PTau range.  All contex
 proof must be the single-context proof of the same key, witness and blinders, byte for byte.  Covered: 1, 2, 3 and 8 ranks
 on the reference fixtures and on chain keys of 2^4 (ranges of a few points; later ranks get empty parts of the shorter
 commitments), 2^10 (plain mode) and 2^14 (window tables), a 2^15 key whose eight ranges mix table and plain mode, forced
-plain mode and MSM chunks smaller than a range, the bench keys at 2^18 and 2^20 against the committed hashes, distinct
-devices when there are several, and the refusals."""
+plain mode, MSM chunks smaller than a range and ranges that end a few points past a chunk, the bench keys at 2^18 and 2^20
+against the committed hashes, distinct devices when there are several, and the refusals."""
 import contextlib
 import functools
 
@@ -118,14 +118,33 @@ def test_ranges_mixing_table_and_plain_mode(ctxs):
     assert sharded_proof(cs, "plonk", zkey, wit, bl) == single_proof(cs[0], "plonk", zkey, wit, bl)
 
 
-@pytest.mark.parametrize("settings", [((3, 1),), ((6, 10),)], ids=["no-tables", "chunks-2^10"])
+def range_past_chunk(lib, points):
+    """(shards, c): the fewest shards, then the largest chunk of 2^c >= 2^10 points, for which rank 0's range of the PTau
+    points (sb_shard_range) ends 1 to 16 points past a chunk boundary"""
+    import ctypes
+    for shards in range(2, 9):
+        first, count = ctypes.c_uint64(), ctypes.c_uint64()
+        lib.sb_shard_range(points, 0, shards, ctypes.byref(first), ctypes.byref(count))
+        for c in range(min(count.value.bit_length() - 1, 23), 9, -1):
+            if 1 <= count.value % (1 << c) <= 16:
+                return shards, c
+    raise AssertionError(f"no shard range of {points} points ends just past a chunk")
+
+
+# "range-past-chunk": the shard count and chunk from range_past_chunk.  The 2^14 keys give PLONK two ranges of 8195 =
+# 2^13 + 3 points and fflonk two of 73737 = 9 * 2^13 + 9 (PTau of n + 6 and 9n + 18 points).
+@pytest.mark.parametrize("settings", [((3, 1),), ((6, 10),), "range-past-chunk"], ids=["no-tables", "chunks-2^10", "range-past-chunk"])
 @pytest.mark.parametrize("proto,cname", [("plonk", "bls12381"), ("fflonk", "bn128")])
 def test_forced_modes(ctxs, proto, cname, settings):
     zkey, wit = key_of(proto, cname, 14)
     cs = ctxs[cname]
     bl = blinders(proto, cs[0].r)
+    shards = 3
+    if settings == "range-past-chunk":
+        shards, c = range_past_chunk(cs[0].lib, (1 << 14) + 6 if proto == "plonk" else (9 << 14) + 18)
+        settings = ((6, c),)
     with tuning(cs[0].lib, settings):
-        got = sharded_proof(cs[:3], proto, zkey, wit, bl)
+        got = sharded_proof(cs[:shards], proto, zkey, wit, bl)
         assert got == single_proof(cs[0], proto, zkey, wit, bl)
     assert got == single_proof(cs[0], proto, zkey, wit, bl)
 

@@ -56,7 +56,14 @@ def test_resident_needs_a_witness():
 def test_bench_workload_at_config_size_matches_committed_cpu_hash(proto, cname, L):
     """BASELINE config #5 at 2^18 and at its stated size 2^20: the proof of the bench key equals the CPU port's, through
     the hash the CPU port committed (tests/golden/bench_proof_hashes.json, made by make_bench_hashes.py; the port needs
-    40 s per 2^20 proof, so it is not re-run here), from a host witness and from the resident one."""
+    40 s per 2^20 proof, so it is not re-run here), from a host witness and from the resident one.
+
+    The same key then proves a batch of three copies of the witness in sub-batches of 2 and 1 (sb_set_tuning(14, 2)),
+    with the bench blinders, other blinders and the bench blinders again: slots 0 and 2 have the committed hash, slot 1
+    is prove_raw's proof, and the resident witness still gives the committed proof.  This runs the batch flow at the
+    configuration sizes: the commitment sort of 3K' rows, the keyed scans and segmented reductions over tens of millions
+    of elements, the sub-batch sized from free memory and the three-pass strided NTTs.  fflonk at 2^20 has rows of
+    9n = 9 * 2^20 > 2^23 points, more than one MSM chunk, so its batch is the unforced run of the row-by-row commitments."""
     import snarkjs_b200
     from snarkjs_b200 import fflonk, plonk, synth
     import bench_plonk as B
@@ -73,6 +80,17 @@ def test_bench_workload_at_config_size_matches_committed_cpu_hash(proto, cname, 
         raw = pk.prove_raw(wit, bl)
         assert proof_hash(mod.proof_to_object(curve, raw)) == want
         assert pk.prove_raw(None, bl) == raw
+        row = (1 << L) + 6 if proto == "plonk" else 9 << L          # points per commitment row of a batch
+        assert (row > 1 << 23) == (proto == "fflonk" and L == 20)   # only fflonk at 2^20 commits row by row unforced
+        bl2 = bl[32:] + bl[:32]
+        try:
+            assert curve.lib.sb_set_tuning(14, 2) == 0
+            got = pk.prove_batch_raw([wit] * 3, [bl, bl2, bl])
+        finally:
+            curve.lib.sb_set_tuning(14, 0)
+        assert got[0] == got[2] == raw
+        assert pk.prove_raw(None, bl) == raw                       # the batch left the resident witness as it was
+        assert got[1] == pk.prove_raw(wit, bl2) != raw
         pk.release()
     finally:
         curve.terminate()
