@@ -137,6 +137,22 @@ int sb_groth16_release(sb_ctx* ctx, uint64_t handle);
  *   public inputs; sb_set_tuning(14) caps them).  count == 0 writes nothing.  sb_last_ms(0) = the whole call. */
 int sb_groth16_verify_batch(sb_ctx* ctx, const uint8_t* vk, uint64_t vk_len, uint32_t n_public,
                             const uint8_t* publics, const uint8_t* proofs, uint32_t count, int32_t* status_out);
+/* plonkVerify (src/plonk_verify.js:29-421) / fflonkVerify (src/fflonk_verify.js:28-597) for count proofs against one
+ * verification key of a circuit with n_public public signals and domain size 2^power.
+ * vk (affine Montgomery points, all-zero = infinity; Fr values Montgomery, 32 bytes each):
+ *   PLONK:  Qm Ql Qr Qo Qc S1 S2 S3 (G1) || X_2 (G2) || k1 || k2 (Fr): 20 n8q + 64 bytes
+ *   fflonk: C0 (G1) || X_2 (G2) || k1 k2 w w3 w4 w8 wr (Fr): 6 n8q + 224 bytes; BN254 only
+ * publics = count * n_public * 32 bytes, plain LE; proofs = count * sb_plonk_proof_bytes / sb_fflonk_proof_bytes, laid out as
+ *   the provers write them (fflonk's inv evaluation is carried but not read).
+ * status_out[k]: 0 verifies, 1 "Invalid Proof", 2 "Public inputs are not valid." (a signal >= r), 3 proof commitments not
+ *   valid (a point off its curve or a coordinate >= q; no subgroup check), 4 proof evaluations not valid (a Montgomery
+ *   evaluation >= r), checked in the order 3, 4, 2, then the pairing.  SB_ERR_ARG: a wrong vk_len, a null buffer, a vk point
+ *   off its curve or with a coordinate >= q, power above the 2-adicity of Fr, fflonk on a BLS12-381 context.  Sub-batches,
+ *   sb_set_tuning(14), count == 0 and sb_last_ms(0) as sb_groth16_verify_batch. */
+int sb_plonk_verify_batch(sb_ctx* ctx, const uint8_t* vk, uint64_t vk_len, uint32_t n_public, uint32_t power,
+                          const uint8_t* publics, const uint8_t* proofs, uint32_t count, int32_t* status_out);
+int sb_fflonk_verify_batch(sb_ctx* ctx, const uint8_t* vk, uint64_t vk_len, uint32_t n_public, uint32_t power,
+                           const uint8_t* publics, const uint8_t* proofs, uint32_t count, int32_t* status_out);
 /* test hook, the device pairing (csrc/pairing.cuh) on the context's curve over n records: op 0 Fq12 mul (a, b), 1 Fq12 square,
  * 2 cyclotomic square, 3 inverse, 4 Frobenius (a -> a^q, a^(q^2), a^(q^3): three outputs), 5 Miller loop of one (G1, G2)
  * pair, 6 final exponentiation, 7 full pairing.  Tower elements are 12 Montgomery Fq coefficients in ffjavascript's order
@@ -321,7 +337,7 @@ double sb_calibrate(sb_ctx* ctx, int what);
  *      registered or a key is loaded; a table keeps the c in force at that moment.  Tables are still skipped when
  *      W * n >= 2^31.  A large c costs memory: a plain MSM allocates W * 2^(c-1) buckets.
  *  14  most proofs per sub-batch of sb_groth16_prove_batch, sb_plonk_prove_batch, sb_fflonk_prove_batch and
- *      sb_groth16_verify_batch, and rows per sub-batch of
+ *      sb_groth16_verify_batch, sb_plonk_verify_batch, sb_fflonk_verify_batch, and rows per sub-batch of
  *      sb_msm_registered_batch (test hook;
  *      0 = default: as many as the 32-bit bucket keys and free device memory allow)
  * The Python mirror applies SB_TUNE="key=value,..." from the environment when it loads the library. */

@@ -51,6 +51,8 @@ _SIGNATURES = {
     "sb_groth16_prove_batch": (ctypes.c_int, [vp, u64, vp, u64, u32, vp, vp, vp]),
     "sb_groth16_release": (ctypes.c_int, [vp, u64]),
     "sb_groth16_verify_batch": (ctypes.c_int, [vp, vp, u64, u32, vp, vp, u32, vp]),
+    "sb_plonk_verify_batch": (ctypes.c_int, [vp, vp, u64, u32, u32, vp, vp, u32, vp]),
+    "sb_fflonk_verify_batch": (ctypes.c_int, [vp, vp, u64, u32, u32, vp, vp, u32, vp]),
     "sb_pairing_eval": (ctypes.c_int, [vp, ctypes.c_int, vp, u64, vp]),
     "sb_plonk_load": (ctypes.c_int, [vp, vp, u64, ctypes.POINTER(u64)]),
     "sb_plonk_load_file": (ctypes.c_int, [vp, ctypes.c_char_p, ctypes.POINTER(u64)]),

@@ -10,7 +10,9 @@
 //                 of its own; normalised with one inversion per point (affine, or Jacobian with Z = 1, infinity (0,1,0))
 // Twiddles and apply-key scalars are plain (non-Montgomery) little-endian Fr values below r < 2^255.
 #pragma once
+#ifdef __CUDACC__
 #include <cuda_runtime.h>
+#endif
 #include "ec.cuh"
 
 namespace sb {
@@ -18,6 +20,8 @@ namespace sb {
 static constexpr int GFFT_THREADS = 128;
 
 struct FrPlain { uint32_t v[8]; };
+
+#ifdef __CUDACC__   // the rest is device code; FrPlain is shared with host builds of the verifiers
 
 // k * p for a plain scalar k < 2^255.  Digits d_i in [-7, 8] with k = sum d_i 16^i: a nibble plus the incoming carry
 // above 8 becomes d - 16 and carries one; the top nibble is at most 7, so no digit 64 is needed.
@@ -129,5 +133,7 @@ template <class F> int gfft_run(const uint8_t* d_in, int in_jac, uint64_t n, int
     *launches = L + 2;
     return (int)cudaGetLastError();
 }
+
+#endif  // __CUDACC__
 
 }  // namespace sb

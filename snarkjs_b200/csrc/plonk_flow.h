@@ -13,31 +13,14 @@
 #include <cstring>
 #include <string>
 #include <vector>
+#include "keccak.cuh"
 #include "plonk.cuh"
 #include "zkey.h"
 
 namespace sb {
 
 // ------------------------------------------------------------------------------------------------ Keccak-256
-// (src/Keccak256Transcript.js:21 uses @noble/hashes keccak_256: Keccak-f[1600], rate 136, domain byte 0x01)
-inline void keccak_f1600(uint64_t* a) {
-    static const uint64_t RC[24] = {0x0000000000000001ull, 0x0000000000008082ull, 0x800000000000808Aull, 0x8000000080008000ull, 0x000000000000808Bull,
-        0x0000000080000001ull, 0x8000000080008081ull, 0x8000000000008009ull, 0x000000000000008Aull, 0x0000000000000088ull, 0x0000000080008009ull,
-        0x000000008000000Aull, 0x000000008000808Bull, 0x800000000000008Bull, 0x8000000000008089ull, 0x8000000000008003ull, 0x8000000000008002ull,
-        0x8000000000000080ull, 0x000000000000800Aull, 0x800000008000000Aull, 0x8000000080008081ull, 0x8000000000008080ull, 0x0000000080000001ull,
-        0x8000000080008008ull};
-    static const int ROT[25] = {0, 1, 62, 28, 27, 36, 44, 6, 55, 20, 3, 10, 43, 25, 39, 41, 45, 15, 21, 8, 18, 2, 61, 56, 14};   // [x + 5y]
-    auto rol = [](uint64_t x, int n) { return n ? (x << n) | (x >> (64 - n)) : x; };
-    for (int round = 0; round < 24; round++) {
-        uint64_t c[5], d[5], b[25];
-        for (int x = 0; x < 5; x++) c[x] = a[x] ^ a[x + 5] ^ a[x + 10] ^ a[x + 15] ^ a[x + 20];
-        for (int x = 0; x < 5; x++) d[x] = c[(x + 4) % 5] ^ rol(c[(x + 1) % 5], 1);
-        for (int i = 0; i < 25; i++) a[i] ^= d[i % 5];
-        for (int x = 0; x < 5; x++) for (int y = 0; y < 5; y++) b[y + 5 * ((2 * x + 3 * y) % 5)] = rol(a[x + 5 * y], ROT[x + 5 * y]);
-        for (int x = 0; x < 5; x++) for (int y = 0; y < 5; y++) a[x + 5 * y] = b[x + 5 * y] ^ (~b[(x + 1) % 5 + 5 * y] & b[(x + 2) % 5 + 5 * y]);
-        a[0] ^= RC[round];
-    }
-}
+// (the permutation is keccak.cuh's, shared with the device verifiers)
 inline void keccak256(const uint8_t* data, size_t len, uint8_t out[32]) {
     const size_t rate = 136;
     std::vector<uint8_t> msg(data, data + len);

@@ -7,7 +7,9 @@
 //                     their curves, else 3), cpub = IC[0] + sum of the proof's terms, one multi-Miller loop over (-A, B),
 //                     (cpub, gamma2), (C, delta2), one final exponentiation, and the comparison with the target (0, else 1).
 #pragma once
+#ifdef __CUDACC__
 #include <cuda_runtime.h>
+#endif
 #include "pairing.cuh"
 #include "gfft.cuh"
 
@@ -52,6 +54,7 @@ template <class P> bool vk_valid_host(const Fp<P>* vk, uint32_t n_public) {
     return ok;
 }
 
+#ifdef __CUDACC__   // kernels; the helpers above are shared with host builds
 template <class P> __global__ void __launch_bounds__(VERIFY_THREADS)
 k_pair_eval(int op, const Fp<P>* __restrict__ in, Fp<P>* __restrict__ out, uint64_t n, int wi, int wo) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -114,5 +117,7 @@ k_verify(const Fp<P>* __restrict__ vk, uint32_t n_public, const PairLine<P>* __r
     const Fq12<P> f = T::miller(ax, F::neg(ay), bx, by, live0, px, py, lines, live1, cx, cy, lines + T::NLINES, live2);
     status[k] = T::eq(T::final_exp(f), *target) ? 0 : 1;
 }
+
+#endif  // __CUDACC__
 
 }  // namespace sb

@@ -182,3 +182,75 @@ def prove_batch(zkey, wtns_list, blinders=None):
     finally:
         if not isinstance(zkey, ProvingKey):
             pk.release()
+
+
+# ------------------------------------------------------------------ verification (src/fflonk_verify.js:28-597)
+# status -> (log level, the reference's message), as plonk.VERIFY_MESSAGES
+VERIFY_MESSAGES = {1: ("warn", "Invalid Proof"), 2: ("error", "Public inputs are not valid."),
+                   3: ("error", "Proof commitments are not valid"), 4: ("error", "Proof evaluations are not valid."),
+                   5: ("error", "Number of public signals does not match with vk")}
+VK_FR = ("k1", "k2", "w", "w3", "w4", "w8", "wr")
+
+
+def verification_key(zkey) -> dict:
+    """zkey export verificationkey for an fflonk key (src/zkey_export_verificationkey.js:119-148), as decimal strings."""
+    from .plonk import _g1_json, _g2_json, _vk_header, fr_root
+    data, z, o = _vk_header(zkey, "fflonk")
+    n8, q, r = z["n8q"], z["q"], z["r"]
+    fr = [str(_from_mont(data[o + 32 * i:o + 32 * (i + 1)], r, 32)) for i in range(6)]   # k1 k2 w3 w4 w8 wr
+    o += 6 * 32
+    vk = {"protocol": "fflonk", "curve": "bn128" if n8 == 32 else "bls12381", "nPublic": z["nPublic"], "power": z["power"],
+          "k1": fr[0], "k2": fr[1], "w": str(fr_root(r, z["power"])), "w3": fr[2], "w4": fr[3], "w8": fr[4], "wr": fr[5],
+          "X_2": _g2_json(data[o:o + 4 * n8], n8, q), "C0": _g1_json(data[o + 4 * n8:o + 6 * n8], n8, q)}
+    return vk
+
+
+def vk_bytes(vk: dict) -> bytes:
+    """The verification key as sb_fflonk_verify_batch takes it: C0 || X_2 || k1 k2 w w3 w4 w8 wr."""
+    from .groth16 import _curve_of, point_bytes
+    from .plonk import fr_bytes
+    n8, q, r, _name = _curve_of(vk["curve"])
+    return point_bytes(vk["C0"], 1, n8, q) + point_bytes(vk["X_2"], 2, n8, q) + b"".join(fr_bytes(vk[k], r) for k in VK_FR)
+
+
+def proof_bytes(proof: dict, n8: int, q: int, r: int) -> bytes:
+    """A JSON proof as sb_fflonk_prove writes it: C1 C2 W1 W2, then the 16 evaluations (Montgomery, as plonk.fr_bytes)."""
+    from .groth16 import point_bytes
+    from .plonk import fr_bytes
+    ev = proof["evaluations"]
+    return (b"".join(point_bytes(proof["polynomials"][k], 1, n8, q) for k in POINTS)
+            + b"".join(fr_bytes(ev.get(k, 0), r) for k in EVALS))
+
+
+def verify_status(vk_verifier: dict, items, curve: Curve | None = None) -> list:
+    """sb_fflonk_verify_batch over [(publicSignals, proof), ...]: one status per item (0 verifies, else a key of
+    VERIFY_MESSAGES).  A C0 that is not on the curve fails every item with 3, as the reference checks vk.C0 per proof."""
+    from .groth16 import _curve_of
+    from .plonk import _g1_valid, _verify_status
+    n8, q, _r, _name = _curve_of(vk_verifier["curve"])
+    vkb = vk_bytes(vk_verifier)
+    if not _g1_valid(vkb[:2 * n8], n8, q):
+        vkb = None
+    return _verify_status("sb_fflonk_verify_batch", vk_verifier, vkb, items, proof_bytes, len(POINTS), True, curve)
+
+
+def verify_batch(vk_verifier: dict, items, logger=None, curve: Curve | None = None) -> list:
+    """fflonkVerify over many (publicSignals, proof) pairs against one verification key, in one device call -> [bool]."""
+    from .plonk import _log_status
+    st = verify_status(vk_verifier, items, curve)
+    for s in st:
+        _log_status(logger, VERIFY_MESSAGES, s, "PROOF VERIFIED SUCCESSFULLY")
+    return [s == 0 for s in st]
+
+
+def verify(vk_verifier: dict, publicSignals, proof: dict, logger=None, curve: Curve | None = None) -> bool:
+    """fflonkVerify(vk_verifier, publicSignals, proof, logger) (src/fflonk_verify.js:28-137): True, or False with the
+    reference's log message.  Two divergences: without a logger the reference throws on a signal count other than
+    nPublic (its logger.error call there is unguarded), and this returns False; an X_2 off its curve raises SbError,
+    because sb_fflonk_verify_batch refuses such a key, where the reference decodes X_2 without checking it and returns a
+    verdict (an invalid C0 is the reference's own per-proof check, status 3).  verify_batch and verify_status raise
+    alike."""
+    from .plonk import _log_status
+    s = verify_status(vk_verifier, [(publicSignals, proof)], curve)[0]
+    _log_status(logger, VERIFY_MESSAGES, s, "PROOF VERIFIED SUCCESSFULLY")
+    return s == 0

@@ -248,3 +248,172 @@ def prove_batch(zkey, wtns_list, blinders=None):
     finally:
         if not isinstance(zkey, ProvingKey):
             pk.release()
+
+
+# ------------------------------------------------------------------ verification (src/plonk_verify.js:29-421)
+# status -> (log level, the reference's message); 5 is the wrappers' own: a signal count other than nPublic never reaches
+# the device, because the C entry takes one n_public for the whole batch
+VERIFY_MESSAGES = {1: ("warn", "Invalid Proof"), 2: ("error", "Public inputs are not valid."),
+                   3: ("error", "Proof commitments are not valid."), 4: ("error", "Proof evaluations are not valid"),
+                   5: ("error", "Invalid number of public inputs")}
+WRONG_COUNT = 5
+
+
+def fr_root(r: int, k: int) -> int:
+    """Fr.w[k] (build/snarkjs.js:12866-12889): nqr = the first non-residue from 2, w[s] = nqr^((r-1)/2^s) for the
+    2-adicity s, w[k] = w[s]^(2^(s-k))."""
+    s = ((r - 1) & -(r - 1)).bit_length() - 1
+    if not 0 <= k <= s:
+        raise SbError(f"power {k} is above the 2-adicity {s} of Fr")
+    nqr = 2
+    while pow(nqr, (r - 1) // 2, r) != r - 1:
+        nqr += 1
+    return pow(nqr, ((r - 1) >> s) << (s - k), r)
+
+
+def fr_bytes(v, r: int) -> bytes:
+    """Fr.fromObject (build/snarkjs.js:13042-13046): the value written into 32 bytes (toRprLE, :198, silently mod 2^256),
+    then toMontgomery, which reduces it mod r.  So a JSON evaluation of eval + r, or eval + 2^256, is eval."""
+    return ((int(v) % (1 << 256)) % r * (1 << 256) % r).to_bytes(32, "little")
+
+
+def _g1_valid(pb: bytes, n8: int, q: int) -> bool:
+    """G1.isValid of affine Montgomery bytes (point_bytes output: coordinates already below q)."""
+    if pb == bytes(2 * n8):
+        return True
+    x, y = _from_mont(pb[:n8], q, n8), _from_mont(pb[n8:], q, n8)
+    return (y * y - x * x * x - (3 if n8 == 32 else 4)) % q == 0
+
+
+def _g1_json(p: bytes, n8: int, q: int) -> list:
+    return ["0", "1", "0"] if p == bytes(2 * n8) else [str(_from_mont(p[:n8], q, n8)), str(_from_mont(p[n8:], q, n8)), "1"]
+
+
+def _g2_json(p: bytes, n8: int, q: int) -> list:
+    if p == bytes(4 * n8):
+        return [["0", "0"], ["1", "0"], ["0", "0"]]
+    f = lambda i: str(_from_mont(p[i * n8:(i + 1) * n8], q, n8))
+    return [[f(0), f(1)], [f(2), f(3)], ["1", "0"]]
+
+
+def _vk_header(zkey, proto: str) -> tuple:
+    """(header dict, byte offset of k1 in section 2) of a PLONK or fflonk zkey."""
+    from .fflonk import read_zkey_header_fflonk
+    data = bytes(zkey)
+    z = read_zkey_header_plonk(data) if proto == "plonk" else read_zkey_header_fflonk(data)
+    secs = read_binfile(data, "zkey", 2)
+    return data, z, secs[2][0] + 8 + z["n8q"] + z["n8r"] + 20
+
+
+def verification_key(zkey) -> dict:
+    """zkey export verificationkey for a PLONK key (src/zkey_export_verificationkey.js:92-117), as decimal strings."""
+    data, z, o = _vk_header(zkey, "plonk")
+    n8, q, r = z["n8q"], z["q"], z["r"]
+    fr = lambda i: str(_from_mont(data[o + 32 * i:o + 32 * (i + 1)], r, 32))
+    vk = {"protocol": "plonk", "curve": "bn128" if n8 == 32 else "bls12381", "nPublic": z["nPublic"], "power": z["power"],
+          "k1": fr(0), "k2": fr(1)}
+    o += 64
+    for i, name in enumerate(("Qm", "Ql", "Qr", "Qo", "Qc", "S1", "S2", "S3")):
+        vk[name] = _g1_json(data[o + 2 * n8 * i:o + 2 * n8 * (i + 1)], n8, q)
+    o += 16 * n8
+    vk["X_2"] = _g2_json(data[o:o + 4 * n8], n8, q)
+    vk["w"] = str(fr_root(r, z["power"]))
+    return vk
+
+
+def vk_bytes(vk: dict) -> bytes:
+    """The verification key as sb_plonk_verify_batch takes it: Qm Ql Qr Qo Qc S1 S2 S3 || X_2 || k1 || k2."""
+    from .groth16 import _curve_of, point_bytes
+    n8, q, r, _name = _curve_of(vk["curve"])
+    return (b"".join(point_bytes(vk[k], 1, n8, q) for k in ("Qm", "Ql", "Qr", "Qo", "Qc", "S1", "S2", "S3"))
+            + point_bytes(vk["X_2"], 2, n8, q) + fr_bytes(vk["k1"], r) + fr_bytes(vk["k2"], r))
+
+
+def proof_bytes(proof: dict, n8: int, q: int, r: int) -> bytes:
+    """A JSON proof as sb_plonk_prove writes it: the nine points, then the six evaluations (Montgomery, as fr_bytes)."""
+    from .groth16 import point_bytes
+    return b"".join(point_bytes(proof[k], 1, n8, q) for k in POINTS) + b"".join(fr_bytes(proof[k], r) for k in EVALS)
+
+
+def _verify_status(fn: str, vk: dict, vkb: bytes | None, items, encode, n_points: int, count_first: bool, curve) -> list:
+    """The statuses of [(publicSignals, proof), ...] for sb_plonk_verify_batch / sb_fflonk_verify_batch (fn).  vkb = None: a
+    key point the reference checks per proof (fflonk's C0) is not valid, so every proof fails with 3.  Items the device
+    call cannot take (a signal count other than nPublic, a signal outside [0, r)) are decided here, with the reference's
+    check order: the count first for fflonk (count_first), after the commitments for PLONK."""
+    from .groth16 import _curve_of, publics_bytes
+    n8, q, r, name = _curve_of(vk["curve"])
+    n_public, power = int(vk["nPublic"]), int(vk["power"])
+    status = [None] * len(items)
+    pubs, prfs, slots = [], [], []
+    for k, (signals, proof) in enumerate(items):
+        prf = encode(proof, n8, q, r)
+        points_ok = lambda: all(_g1_valid(prf[2 * n8 * i:2 * n8 * (i + 1)], n8, q) for i in range(n_points))
+        if count_first and len(signals) != n_public:
+            status[k] = WRONG_COUNT
+        elif vkb is None:
+            status[k] = 3
+        elif len(signals) != n_public:
+            status[k] = WRONG_COUNT if points_ok() else 3
+        else:
+            pb = publics_bytes(signals, r)
+            if pb is None:                    # evaluations from JSON are always below r (fr_bytes), so 4 cannot come first
+                status[k] = 2 if points_ok() else 3
+            else:
+                pubs.append(pb)
+                prfs.append(prf)
+                slots.append(k)
+    if not slots:
+        return status
+    own = curve is None
+    cv = curve or Curve(name)
+    try:
+        count = len(slots)
+        out = np.zeros(count, np.int32)
+        key = np.frombuffer(vkb, np.uint8)
+        pub = np.frombuffer(b"".join(pubs) or b"\0", np.uint8)
+        prf = np.frombuffer(b"".join(prfs), np.uint8)
+        cv.check(getattr(cv.lib, fn)(cv.handle, _ptr(key), key.size, n_public, power, _ptr(pub), _ptr(prf), count,
+                                     out.ctypes.data_as(ctypes.c_void_p)))
+    finally:
+        if own:
+            cv.terminate()
+    for j, k in enumerate(slots):
+        status[k] = int(out[j])
+    return status
+
+
+def _log_status(logger, messages: dict, s: int, ok: str):
+    if not logger:
+        return
+    if s == 0:
+        logger.info(ok)
+        return
+    if s != 1:
+        logger.error(messages[s][1])
+    else:
+        getattr(logger, messages[1][0])(messages[1][1])
+
+
+def verify_status(vk_verifier: dict, items, curve: Curve | None = None) -> list:
+    """sb_plonk_verify_batch over [(publicSignals, proof), ...]: one status per item (0 verifies, else a key of
+    VERIFY_MESSAGES)."""
+    return _verify_status("sb_plonk_verify_batch", vk_verifier, vk_bytes(vk_verifier), items, proof_bytes, len(POINTS), False, curve)
+
+
+def verify_batch(vk_verifier: dict, items, logger=None, curve: Curve | None = None) -> list:
+    """plonkVerify over many (publicSignals, proof) pairs against one verification key, in one device call -> [bool]."""
+    st = verify_status(vk_verifier, items, curve)
+    for s in st:
+        _log_status(logger, VERIFY_MESSAGES, s, "OK!")
+    return [s == 0 for s in st]
+
+
+def verify(vk_verifier: dict, publicSignals, proof: dict, logger=None, curve: Curve | None = None) -> bool:
+    """plonkVerify(vk_verifier, publicSignals, proof, logger) (src/plonk_verify.js:29-124): True, or False with the
+    reference's log message.  Two divergences: without a logger the reference throws on invalid commitments (its
+    logger.error call there is unguarded), and this returns False; a key point (Qm .. S3, X_2) off its curve raises
+    SbError, because sb_plonk_verify_batch refuses such a key, where the reference decodes the key without checking it
+    and returns a verdict.  verify_batch and verify_status raise alike."""
+    s = verify_status(vk_verifier, [(publicSignals, proof)], curve)[0]
+    _log_status(logger, VERIFY_MESSAGES, s, "OK!")
+    return s == 0
