@@ -258,6 +258,37 @@ int sb_plonk_prove_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, co
 int sb_fflonk_load_multi(sb_ctx* const* ctxs, int n, const uint8_t* zkey, uint64_t zkey_len, uint64_t* handles_out);
 int sb_fflonk_prove_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, const uint8_t* witness, uint64_t n_witness,
                           const uint8_t* blinders, uint8_t* proof_out);
+/* ---- a batch of proofs of one key on several devices --------------------------------------------------------------------
+ * sb_*_load_replicas: the whole key is loaded on each of n in 1..64 distinct contexts, as sb_*_load would, on parallel host
+ *   threads (each under its context's lock).  If a context fails, the handles already made are released and the call returns
+ *   that context's code, with its message on ctxs[0].  Each handle is a complete key: sb_*_prove, sb_*_prove_resident,
+ *   sb_*_prove_batch and sb_*_info take it on its own context, and sb_*_release(ctxs[i], handles[i]) frees it alone.
+ *   sb_*_prove_multi with n > 1 refuses it (SB_ERR_ARG).
+ * sb_*_prove_batch_multi: handles[i] = handles_out[i] of one sb_*_load_replicas call with the same contexts in the same
+ *   order; witnesses, r / s or blinders, proofs_out and status_out (may be NULL) as for sb_*_prove_batch.
+ * - Null pointers, n outside 1..64, a context given twice, contexts of different curves, and handles of another load (plain,
+ *   sharded, another replicas call) or in another order give SB_ERR_ARG before any device work.  A wrong n_witness gives
+ *   the single batch's "Invalid witness length..." text; count == 0 then writes nothing and returns SB_OK.
+ * - The call holds every context's lock for its duration.  Rank i proves the contiguous range sb_shard_range(count, i, n) of
+ *   the proofs with sb_*_prove_batch's device path on a host thread of its own (its sub-batches sized from its own device's
+ *   free memory and sb_set_tuning(14)); a Groth16 rank's host work runs on max(1, cores / n) threads.  Contexts may share
+ *   one device: they run on their own streams.
+ * - Proof k is byte-identical to sb_*_prove_batch on one context with the same inputs.  PLONK / fflonk: a refused proof's
+ *   slot is zero-filled and its status set as in sb_*_prove_batch; the call then returns SB_ERR_ARG and sb_last_error(ctxs[0])
+ *   holds the text of the lowest-index refused proof.  Any other failure of a rank (a CUDA error, SB_ERR_NOMEM) is returned
+ *   with that rank's message on ctxs[0], the lowest rank first, and status_out is not written.
+ * - The resident witness of every context is left as it was.  sb_last_ms(ctxs[0], 0) = the host wall clock of the whole
+ *   call; sb_last_ms(ctxs[i], 0), i > 0 = rank i's own batch time (0 for an empty range).  With n = 1 the call is
+ *   sb_*_prove_batch. */
+int sb_groth16_load_replicas(sb_ctx* const* ctxs, int n, const uint8_t* zkey, uint64_t zkey_len, uint64_t* handles_out);
+int sb_plonk_load_replicas(sb_ctx* const* ctxs, int n, const uint8_t* zkey, uint64_t zkey_len, uint64_t* handles_out);
+int sb_fflonk_load_replicas(sb_ctx* const* ctxs, int n, const uint8_t* zkey, uint64_t zkey_len, uint64_t* handles_out);
+int sb_groth16_prove_batch_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, const uint8_t* witnesses,
+                                 uint64_t n_witness, uint32_t count, const uint8_t* r, const uint8_t* s, uint8_t* proofs_out);
+int sb_plonk_prove_batch_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, const uint8_t* witnesses,
+                               uint64_t n_witness, uint32_t count, const uint8_t* blinders, uint8_t* proofs_out, int32_t* status_out);
+int sb_fflonk_prove_batch_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, const uint8_t* witnesses,
+                                uint64_t n_witness, uint32_t count, const uint8_t* blinders, uint8_t* proofs_out, int32_t* status_out);
 /* multi-GPU: this rank proves with its shard [shard, n_shards) of every MSM and returns the five un-normalised
  * MSM partials (A, B1, C, H in G1; B2 in G2) instead of a proof; the ranks exchange them (NCCL all-gather) and any
  * rank finishes with sb_groth16_finish. */

@@ -74,6 +74,12 @@ _SIGNATURES = {
     "sb_plonk_prove_multi": (ctypes.c_int, [ctypes.POINTER(vp), ctypes.POINTER(u64), ctypes.c_int, vp, u64, ctypes.c_char_p, vp]),
     "sb_fflonk_load_multi": (ctypes.c_int, [ctypes.POINTER(vp), ctypes.c_int, vp, u64, ctypes.POINTER(u64)]),
     "sb_fflonk_prove_multi": (ctypes.c_int, [ctypes.POINTER(vp), ctypes.POINTER(u64), ctypes.c_int, vp, u64, ctypes.c_char_p, vp]),
+    "sb_groth16_load_replicas": (ctypes.c_int, [ctypes.POINTER(vp), ctypes.c_int, vp, u64, ctypes.POINTER(u64)]),
+    "sb_plonk_load_replicas": (ctypes.c_int, [ctypes.POINTER(vp), ctypes.c_int, vp, u64, ctypes.POINTER(u64)]),
+    "sb_fflonk_load_replicas": (ctypes.c_int, [ctypes.POINTER(vp), ctypes.c_int, vp, u64, ctypes.POINTER(u64)]),
+    "sb_groth16_prove_batch_multi": (ctypes.c_int, [ctypes.POINTER(vp), ctypes.POINTER(u64), ctypes.c_int, vp, u64, u32, vp, vp, vp]),
+    "sb_plonk_prove_batch_multi": (ctypes.c_int, [ctypes.POINTER(vp), ctypes.POINTER(u64), ctypes.c_int, vp, u64, u32, vp, vp, vp]),
+    "sb_fflonk_prove_batch_multi": (ctypes.c_int, [ctypes.POINTER(vp), ctypes.POINTER(u64), ctypes.c_int, vp, u64, u32, vp, vp, vp]),
     "sb_groth16_prove_resident": (ctypes.c_int, [vp, u64, vp, vp, vp]),
     "sb_last_stat": (ctypes.c_double, [vp, ctypes.c_int]),
     "sb_calibrate": (ctypes.c_double, [vp, ctypes.c_int]),

@@ -75,6 +75,8 @@ struct Groth16Key {
     MsmGeom gpW{}, gpH{};                                                                // their geometry (precomp != 0 when built)
     // sharded load (multi-GPU): only the point ranges [wlo, wlo+wcnt) of A/B1/B2/C and [hlo, hlo+hcnt) of H are resident
     int shard = 0, n_shards = 1; uint64_t wlo = 0, wcnt = 0, hlo = 0, hcnt = 0;
+    // a whole key made by sb_groth16_load_replicas call replica_id (0: any other load), on context `replica` of n_replicas
+    uint64_t replica_id = 0; int replica = 0, n_replicas = 0;
     uint64_t* d_rowptr = nullptr; uint32_t* d_sig = nullptr; void* d_coef = nullptr; uint64_t nCoef = 0;
     // device work buffers
     bool witness_resident = false;   // set by the first upload: sb_groth16_prove_resident refuses to run before it
@@ -1610,8 +1612,9 @@ static int groth16_prove_batch_chunked(sb_ctx* c, Groth16Key* k, const uint8_t* 
     return 0;
 }
 
+// host_threads: the host pool's size, 0 = one thread per core (a multi-context batch gives each rank its share of the cores)
 static int groth16_prove_batch_impl(sb_ctx* c, Groth16Key* k, const uint8_t* witnesses, uint32_t count,
-                                    const uint8_t* r, const uint8_t* s, uint8_t* proofs) {
+                                    const uint8_t* r, const uint8_t* s, uint8_t* proofs, unsigned host_threads = 0) {
     cudaSetDevice(c->device);
     const uint64_t n = k->domainSize, nv = k->nVars;
     const uint64_t MAXC = 1ull << (g_msm_chunk_log > 0 ? g_msm_chunk_log : 23);
@@ -1631,7 +1634,7 @@ static int groth16_prove_batch_impl(sb_ctx* c, Groth16Key* k, const uint8_t* wit
     const VkPoints vk{k->alpha1.data(), k->beta1.data(), k->beta2.data(), k->delta1.data(), k->delta2.data()};
     // Host work on one pool of at most one thread per core, declared after everything its tasks touch: leaving this
     // function (also on an error) runs the queued tasks and joins.  The fixed parts go first, so they overlap the GPU work.
-    HostPool pool(std::min<unsigned>(count, std::max(1u, std::thread::hardware_concurrency())));
+    HostPool pool(std::min<unsigned>(count, host_threads ? host_threads : std::max(1u, std::thread::hardware_concurrency())));
     for (uint32_t i = 0; i < count; i++)
         pool.submit([&, i]() { fixed[i] = groth16_fixed_parts(cv, G1, G2, vk, r + 32 * (size_t)i, s + 32 * (size_t)i, false); });
     int rc;
@@ -1776,6 +1779,12 @@ int sb_groth16_prove_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, 
                            const uint8_t r[32], const uint8_t s[32], uint8_t* proof_affine_out) {
     if (!ctxs || !handles || n < 1 || !proof_affine_out) return SB_ERR_ARG;
     if (n == 1) return sb_groth16_prove(ctxs[0], handles[0], witness, n_witness, r, s, proof_affine_out);
+    for (int i = 0; i < n; i++) {   // before any rank enters the collective: a refusal on some ranks only would leave the others waiting
+        SB_LOCK(ctxs[i]);
+        const Groth16Key* k = get_key(ctxs[i], handles[i]);
+        if (k && k->replica_id) return fail(ctxs[0], SB_ERR_ARG, "sb_groth16_prove_multi: the key of rank " + std::to_string(i) +
+                                                                     " is a replica of sb_groth16_load_replicas: prove with sb_groth16_prove_batch_multi");
+    }
     std::vector<std::future<int>> f;
     for (int i = 0; i < n; i++)
         f.push_back(std::async(std::launch::async, [=]() { return sb_groth16_prove_dist(ctxs[i], handles[i], witness, n_witness, r, s, i == 0 ? proof_affine_out : nullptr); }));
@@ -1861,8 +1870,9 @@ static int multi_ctx_args(sb_ctx* const* ctxs, int n, const char* name) {
     return 0;
 }
 
+// id numbers the call (g_multi_loads).  sb_*_load_replicas passes peer = false: its ranks never copy between devices.
 static int load_multi(sb_ctx* const* ctxs, int n, uint64_t* handles, const std::function<int(sb_ctx*, int, uint64_t, uint64_t*)>& load,
-                      int (*release)(sb_ctx*, uint64_t), const char* name) {
+                      int (*release)(sb_ctx*, uint64_t), const char* name, bool peer = true) {
     if (int rc = multi_ctx_args(ctxs, n, name)) return rc;
     if (!handles) return fail(ctxs[0], SB_ERR_ARG, "null argument");
     for (int i = 0; i < n; i++) handles[i] = 0;
@@ -1873,10 +1883,10 @@ static int load_multi(sb_ctx* const* ctxs, int n, uint64_t* handles, const std::
             sb_ctx* c = ctxs[i];
             SB_LOCK(c);
             cudaSetDevice(c->device);
-            int rc = load(c, i, n > 1 ? id : 0, &handles[i]);
+            int rc = load(c, i, id, &handles[i]);
             const int d0 = ctxs[0]->device;
             int can = 0;
-            if (!rc && c->device != d0 && cudaDeviceCanAccessPeer(&can, c->device, d0) == cudaSuccess && can) {
+            if (!rc && peer && c->device != d0 && cudaDeviceCanAccessPeer(&can, c->device, d0) == cudaSuccess && can) {
                 cudaError_t e = cudaDeviceEnablePeerAccess(d0, 0);
                 if (e != cudaSuccess && e != cudaErrorPeerAccessAlreadyEnabled) rc = cuda_fail(c, e, "cudaDeviceEnablePeerAccess");
                 cudaGetLastError();
@@ -1894,12 +1904,22 @@ static int load_multi(sb_ctx* const* ctxs, int n, uint64_t* handles, const std::
     return 0;
 }
 
-// Argument checks of sb_*_prove_multi, before any device work: pointers, n, distinct contexts of one curve.  Then every
-// context is locked (in address order, so that calls on overlapping sets of contexts cannot deadlock) and the handles
-// are checked: keys[i] = rank i of one multi load (n = 1: a single-device key).
+// Whether keys[i] = k is rank i of the load keys[0] = k0 belongs to: one sb_*_load_multi call (n = 1: a single-device key),
+// or one sb_*_load_replicas call.
+template <class K> static bool multi_rank(const K* k, const K* k0, int i, int n) {
+    return n == 1 ? k->multi_id == 0 : (k->multi_id && k->multi_id == k0->multi_id && k->rank == i && k->n_ranks == n);
+}
+template <class K> static bool replica_rank(const K* k, const K* k0, int i, int n) {
+    return k->replica_id && k->replica_id == k0->replica_id && k->replica == i && k->n_replicas == n;
+}
+
+// Argument checks of sb_*_prove_multi and sb_*_prove_batch_multi, before any device work: pointers, n, distinct contexts of
+// one curve.  Then every context is locked (in address order, so that calls on overlapping sets of contexts cannot
+// deadlock) and the handles are checked: same_load(keys[i], keys[0], i, n) for every rank.
 template <class K> static int prove_multi_args(sb_ctx* const* ctxs, const uint64_t* handles, int n, const void* witness, const void* blinders,
                                                const void* proof, K* (*get)(sb_ctx*, uint64_t), const char* name,
-                                               std::vector<std::unique_lock<std::recursive_mutex>>& locks, std::vector<K*>& keys) {
+                                               std::vector<std::unique_lock<std::recursive_mutex>>& locks, std::vector<K*>& keys,
+                                               bool (*same_load)(const K*, const K*, int, int) = multi_rank<K>, const char* load = "load_multi") {
     if (int rc = multi_ctx_args(ctxs, n, name)) return rc;
     sb_ctx* c0 = ctxs[0];
     if (!handles || !witness || !blinders || !proof) return fail(c0, SB_ERR_ARG, "null argument");
@@ -1913,12 +1933,45 @@ template <class K> static int prove_multi_args(sb_ctx* const* ctxs, const uint64
         keys[i] = get(ctxs[i], handles[i]);
         if (!keys[i]) return fail(c0, SB_ERR_ARG, std::string(name) + ": invalid handle of rank " + std::to_string(i));
     }
-    for (int i = 0; i < n; i++) {
-        const K* k = keys[i];
-        const bool ok = n == 1 ? k->multi_id == 0 : (k->multi_id && k->multi_id == keys[0]->multi_id && k->rank == i && k->n_ranks == n);
-        if (!ok) return fail(c0, SB_ERR_ARG, std::string(name) + ": the handles do not come from one load_multi call of these " + std::to_string(n) + " contexts, in this order");
-    }
+    for (int i = 0; i < n; i++)
+        if (!same_load(keys[i], keys[0], i, n))
+            return fail(c0, SB_ERR_ARG, std::string(name) + ": the handles do not come from one " + load + " call of these " + std::to_string(n) + " contexts, in this order");
     return 0;
+}
+
+// sb_*_prove_batch_multi after its argument checks, with every context locked: rank i proves the proofs
+// [lo, lo + cnt) = sb_shard_range(count, i, n) with prove(i, lo, cnt, statuses of those proofs or null) on a host thread of
+// its own.  with_status (PLONK / fflonk): the per-proof statuses are collected and copied to status_out (when not null)
+// unless a rank failed for another reason than refused proofs.  Returns 0; or the lowest such rank's code, with its message
+// on ctxs[0]; or SB_ERR_ARG with the text of the lowest-index refused proof, which is the message of the lowest rank that
+// refused one (each rank reports its own lowest).  sb_last_ms(ctxs[0], 0) = the host wall clock of the call;
+// sb_last_ms(ctxs[i], 0), i > 0 = rank i's batch (0 for an empty range).
+static int batch_multi_run(sb_ctx* const* ctxs, int n, uint32_t count, bool with_status, int32_t* status_out,
+                           const std::function<int(int, uint32_t, uint32_t, int32_t*)>& prove) {
+    const auto t0 = std::chrono::steady_clock::now();
+    std::vector<int32_t> status(with_status ? count : 0, 0);
+    std::vector<std::future<int>> f;
+    for (int i = 0; i < n; i++)
+        f.push_back(std::async(std::launch::async, [&, i]() {
+            uint64_t lo, cnt; sb_shard_range(count, i, n, &lo, &cnt);
+            ctxs[i]->last_ms[0] = 0;
+            if (!cnt) return 0;
+            cudaSetDevice(ctxs[i]->device);
+            return prove(i, (uint32_t)lo, (uint32_t)cnt, with_status ? status.data() + lo : nullptr);
+        }));
+    std::vector<int> rcs(n);
+    for (int i = 0; i < n; i++) rcs[i] = f[i].get();
+    ctxs[0]->last_ms[0] = std::chrono::duration<float, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    int refused = -1;
+    for (int i = 0; i < n; i++) {
+        if (!rcs[i]) continue;
+        uint64_t lo, cnt; sb_shard_range(count, i, n, &lo, &cnt);
+        const bool any = with_status && std::any_of(status.begin() + lo, status.begin() + lo + cnt, [](int32_t s) { return s != 0; });
+        if (rcs[i] != SB_ERR_ARG || !any) return fail(ctxs[0], rcs[i], ctxs[i]->err);
+        if (refused < 0) refused = i;
+    }
+    if (status_out) memcpy(status_out, status.data(), status.size() * sizeof(int32_t));
+    return refused < 0 ? 0 : fail(ctxs[0], SB_ERR_ARG, ctxs[refused]->err);
 }
 
 extern "C" {
@@ -2040,8 +2093,8 @@ int sb_fflonk_release(sb_ctx* c, uint64_t h) { SB_LOCK(c);
 int sb_plonk_load_multi(sb_ctx* const* ctxs, int n, const uint8_t* zkey, uint64_t zkey_len, uint64_t* handles) {
     if (!zkey) return SB_ERR_ARG;
     return load_multi(ctxs, n, handles, [=](sb_ctx* c, int i, uint64_t id, uint64_t* h) {
-        return c->curve == SB_BN254 ? plonk_load_impl<BnFr>(c, zkey, zkey_len, h, i, id ? n : 1, id)
-                                    : plonk_load_impl<BlsFr>(c, zkey, zkey_len, h, i, id ? n : 1, id);
+        return c->curve == SB_BN254 ? plonk_load_impl<BnFr>(c, zkey, zkey_len, h, i, n, n > 1 ? id : 0)
+                                    : plonk_load_impl<BlsFr>(c, zkey, zkey_len, h, i, n, n > 1 ? id : 0);
     }, sb_plonk_release, "sb_plonk_load_multi");
 }
 int sb_plonk_prove_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, const uint8_t* witness, uint64_t n_witness,
@@ -2064,7 +2117,7 @@ int sb_fflonk_load_multi(sb_ctx* const* ctxs, int n, const uint8_t* zkey, uint64
     if (!zkey) return SB_ERR_ARG;
     return load_multi(ctxs, n, handles, [=](sb_ctx* c, int i, uint64_t id, uint64_t* h) {
         if (c->curve != SB_BN254) return fail(c, SB_ERR_ARG, "fflonk is defined on bn128 only (src/fflonk_setup.js:534-557)");
-        return fflonk_load_impl<BnFr>(c, zkey, zkey_len, h, i, id ? n : 1, id);
+        return fflonk_load_impl<BnFr>(c, zkey, zkey_len, h, i, n, n > 1 ? id : 0);
     }, sb_fflonk_release, "sb_fflonk_load_multi");
 }
 int sb_fflonk_prove_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, const uint8_t* witness, uint64_t n_witness,
@@ -2082,6 +2135,93 @@ int sb_fflonk_prove_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, c
     rc = fflonk_prove_impl<BnFq, BnFr>(c, keys[0], witness, n_witness, blinders, proof, be);
     cudaEventDestroy(rk.ready);
     return rc;
+}
+
+}  // extern "C"
+
+// ---- batches of one key on several devices (sb_*_load_replicas, sb_*_prove_batch_multi)
+// sb_*_load_replicas: load_multi with the whole key on every context, each handle marked as replica i of the call.
+template <class K> static int load_replicas(sb_ctx* const* ctxs, int n, uint64_t* handles, const std::function<int(sb_ctx*, uint64_t*)>& load,
+                                            std::vector<K*> sb_ctx::*keys, int (*release)(sb_ctx*, uint64_t), const char* name) {
+    return load_multi(ctxs, n, handles, [&](sb_ctx* c, int i, uint64_t id, uint64_t* h) {
+        int rc = load(c, h);
+        if (!rc) { K* k = (c->*keys)[*h - 1]; k->replica_id = id; k->replica = i; k->n_replicas = n; }
+        return rc;
+    }, release, name, false);
+}
+
+extern "C" {
+
+int sb_groth16_load_replicas(sb_ctx* const* ctxs, int n, const uint8_t* zkey, uint64_t zkey_len, uint64_t* handles) {
+    if (!zkey) return SB_ERR_ARG;
+    return load_replicas<Groth16Key>(ctxs, n, handles, [=](sb_ctx* c, uint64_t* h) { return groth16_load_impl(c, zkey, zkey_len, 0, 1, h); },
+                                     &sb_ctx::keys, sb_groth16_release, "sb_groth16_load_replicas");
+}
+int sb_plonk_load_replicas(sb_ctx* const* ctxs, int n, const uint8_t* zkey, uint64_t zkey_len, uint64_t* handles) {
+    if (!zkey) return SB_ERR_ARG;
+    return load_replicas<PlonkKeyDev>(ctxs, n, handles, [=](sb_ctx* c, uint64_t* h) { return sb_plonk_load(c, zkey, zkey_len, h); },
+                                      &sb_ctx::plonk_keys, sb_plonk_release, "sb_plonk_load_replicas");
+}
+int sb_fflonk_load_replicas(sb_ctx* const* ctxs, int n, const uint8_t* zkey, uint64_t zkey_len, uint64_t* handles) {
+    if (!zkey) return SB_ERR_ARG;
+    return load_replicas<FflonkKeyDev>(ctxs, n, handles, [=](sb_ctx* c, uint64_t* h) { return sb_fflonk_load(c, zkey, zkey_len, h); },
+                                       &sb_ctx::fflonk_keys, sb_fflonk_release, "sb_fflonk_load_replicas");
+}
+
+int sb_groth16_prove_batch_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, const uint8_t* witnesses, uint64_t n_witness,
+                                 uint32_t count, const uint8_t* r, const uint8_t* s, uint8_t* proofs) {
+    std::vector<std::unique_lock<std::recursive_mutex>> locks; std::vector<Groth16Key*> keys;
+    int rc = prove_multi_args(ctxs, handles, n, witnesses, r && s ? r : nullptr, proofs, get_key, "sb_groth16_prove_batch_multi", locks, keys,
+                              replica_rank<Groth16Key>, "load_replicas");
+    if (rc) return rc;
+    sb_ctx* c = ctxs[0];
+    if (n == 1) return sb_groth16_prove_batch(c, handles[0], witnesses, n_witness, count, r, s, proofs);
+    if (n_witness != keys[0]->nVars) return fail(c, SB_ERR_ARG, "Invalid witness length. Circuit: " + std::to_string(keys[0]->nVars) + ", witness: " + std::to_string(n_witness));
+    if (count == 0) return SB_OK;
+    // the ranks' host pools share the cores
+    const unsigned threads = std::max(1u, std::thread::hardware_concurrency() / n);
+    const size_t pb = 2 * c->g1.aff_bytes + c->g2.aff_bytes;
+    return batch_multi_run(ctxs, n, count, false, nullptr, [&](int i, uint32_t lo, uint32_t cnt, int32_t*) {
+        return groth16_prove_batch_impl(ctxs[i], keys[i], witnesses + (size_t)lo * n_witness * 32, cnt, r + (size_t)lo * 32, s + (size_t)lo * 32,
+                                        proofs + lo * pb, threads);
+    });
+}
+int sb_plonk_prove_batch_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, const uint8_t* witnesses, uint64_t n_witness,
+                               uint32_t count, const uint8_t* blinders, uint8_t* proofs, int32_t* status) {
+    std::vector<std::unique_lock<std::recursive_mutex>> locks; std::vector<PlonkKeyDev*> keys;
+    int rc = prove_multi_args(ctxs, handles, n, witnesses, blinders, proofs, get_plonk_key, "sb_plonk_prove_batch_multi", locks, keys,
+                              replica_rank<PlonkKeyDev>, "load_replicas");
+    if (rc) return rc;
+    sb_ctx* c = ctxs[0];
+    if (n == 1) return sb_plonk_prove_batch(c, handles[0], witnesses, n_witness, count, blinders, proofs, status);
+    const PlonkZkey& z = keys[0]->z;
+    if (n_witness != (uint64_t)z.nVars - z.nAdditions)
+        return fail(c, SB_ERR_ARG, "Invalid witness length. Circuit: " + std::to_string(z.nVars) + ", witness: " + std::to_string(n_witness) + ", " + std::to_string(z.nAdditions));
+    if (count == 0) return SB_OK;
+    const size_t pb = sb_plonk_proof_bytes(c);
+    return batch_multi_run(ctxs, n, count, true, status, [&](int i, uint32_t lo, uint32_t cnt, int32_t* st) {
+        const uint8_t* w = witnesses + (size_t)lo * n_witness * 32; const uint8_t* b = blinders + (size_t)lo * 11 * 32;
+        return c->curve == SB_BN254 ? plonk_prove_batch_impl<BnFq, BnFr>(ctxs[i], keys[i], w, n_witness, cnt, b, proofs + lo * pb, st)
+                                    : plonk_prove_batch_impl<BlsFq, BlsFr>(ctxs[i], keys[i], w, n_witness, cnt, b, proofs + lo * pb, st);
+    });
+}
+int sb_fflonk_prove_batch_multi(sb_ctx* const* ctxs, const uint64_t* handles, int n, const uint8_t* witnesses, uint64_t n_witness,
+                                uint32_t count, const uint8_t* blinders, uint8_t* proofs, int32_t* status) {
+    std::vector<std::unique_lock<std::recursive_mutex>> locks; std::vector<FflonkKeyDev*> keys;
+    int rc = prove_multi_args(ctxs, handles, n, witnesses, blinders, proofs, get_fflonk_key, "sb_fflonk_prove_batch_multi", locks, keys,
+                              replica_rank<FflonkKeyDev>, "load_replicas");
+    if (rc) return rc;
+    sb_ctx* c = ctxs[0];
+    if (n == 1) return sb_fflonk_prove_batch(c, handles[0], witnesses, n_witness, count, blinders, proofs, status);
+    const FflonkZkey& z = keys[0]->z;
+    if (n_witness != (uint64_t)z.nVars - z.nAdditions)
+        return fail(c, SB_ERR_ARG, "Invalid witness length. Circuit: " + std::to_string(z.nVars) + ", witness: " + std::to_string(n_witness) + ", " + std::to_string(z.nAdditions));
+    if (count == 0) return SB_OK;
+    const size_t pb = sb_fflonk_proof_bytes(c);
+    return batch_multi_run(ctxs, n, count, true, status, [&](int i, uint32_t lo, uint32_t cnt, int32_t* st) {
+        return fflonk_prove_batch_impl<BnFq, BnFr>(ctxs[i], keys[i], witnesses + (size_t)lo * n_witness * 32, n_witness, cnt,
+                                                   blinders + (size_t)lo * 9 * 32, proofs + lo * pb, st);
+    });
 }
 
 }  // extern "C"

@@ -13,7 +13,9 @@ import numpy as np
 
 from .curve import Curve, SbError, _arr, _ptr, getCurveFromQ
 from .groth16 import _from_mont, random_fr, read_binfile, read_wtns_header
+from .plonk import ReplicatedProvingKey as _PlonkReplicated
 from .plonk import ShardedProvingKey as _PlonkSharded
+from .plonk import _prove_batch
 
 POINTS = ("C1", "C2", "W1", "W2")
 EVALS = ("ql", "qr", "qm", "qo", "qc", "s1", "s2", "s3", "a", "b", "c", "z", "zw", "t1w", "t2w", "inv")
@@ -95,29 +97,8 @@ class ProvingKey:
         """One sb_fflonk_prove_batch call: witnesses = wtns section-2 payloads ((nVars - nAdditions) x 32 bytes each),
         blinders_list = one 9 x 32-byte Montgomery blinder string per witness.  Returns one proof (bytes, as prove_raw) per
         witness, or None for a proof the reference would have rejected; raises SbError for argument and device errors."""
-        parts = [_arr(x) for x in witnesses]
-        count = len(parts)
-        if len(blinders_list) != count:
-            raise SbError("one blinder set per witness")
-        if count == 0:
-            return []
-        for b in blinders_list:
-            if len(b) != 9 * 32:
-                raise SbError("blinders must be 9 field elements")
-        n_wit = parts[0].size // 32
-        for x in parts:
-            if x.size != parts[0].size:
-                raise SbError("witnesses of one batch must have the same length")
-        lib, c = self.curve.lib, self.curve
-        w = np.concatenate(parts)
-        bl = np.frombuffer(b"".join(bytes(b) for b in blinders_list), np.uint8)
-        pb = lib.sb_fflonk_proof_bytes(c.handle)
-        out = np.empty(count * pb, np.uint8)
-        status = np.zeros(count, np.int32)
-        rc = lib.sb_fflonk_prove_batch(c.handle, self.handle, _ptr(w), n_wit, count, _ptr(bl), _ptr(out), _ptr(status))
-        if rc != 0 and not status.any():
-            c.check(rc)
-        return [None if status[i] else out[i * pb:(i + 1) * pb].tobytes() for i in range(count)]
+        return _prove_batch(self.curve, "fflonk", 9, witnesses, blinders_list,
+                            lambda w, n_wit, count, bl, out, st: self.curve.lib.sb_fflonk_prove_batch(self.curve.handle, self.handle, w, n_wit, count, bl, out, st))
 
     def release(self):
         if self.handle:
@@ -135,6 +116,14 @@ class ShardedProvingKey(_PlonkSharded):
     PROTO, N_BLINDERS = "fflonk", 9
     read_header = staticmethod(read_zkey_header_fflonk)
     to_object = staticmethod(proof_to_object)
+
+
+class ReplicatedProvingKey(_PlonkReplicated):
+    """An fflonk zkey loaded whole on several contexts (sb_fflonk_load_replicas), so that a batch of proofs is split over
+    them (sb_fflonk_prove_batch_multi), with the interface of plonk.ReplicatedProvingKey."""
+
+    PROTO, N_BLINDERS = "fflonk", 9
+    read_header = staticmethod(read_zkey_header_fflonk)
 
 
 def prove(zkey, wtns: bytes, blinders: bytes | None = None, logger=None, options=None):

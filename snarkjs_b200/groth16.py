@@ -102,6 +102,95 @@ def proof_to_object(curve: Curve, affine: bytes) -> dict:
     return {"pi_a": g1(a), "pi_b": g2(b), "pi_c": g1(c), "protocol": "groth16", "curve": curve.name}
 
 
+def _batch_inputs(n_vars: int, witnesses, rs):
+    """(witnesses back to back, r's, s's, count) from prove_batch_raw's arguments, checked as the batch entries need them."""
+    count = len(rs)
+    if isinstance(witnesses, (list, tuple)):
+        if len(witnesses) != count:
+            raise SbError(f"{len(witnesses)} witnesses but {count} (r, s) pairs")
+        parts = [_arr(x) for x in witnesses]
+        for x in parts:
+            if x.size != 32 * n_vars:
+                raise SbError(f"Invalid witness length. Circuit: {n_vars}, witness: {x.size // 32}")
+        w = np.concatenate(parts) if parts else np.zeros(0, np.uint8)
+    else:
+        w = _arr(witnesses)
+        if w.size != 32 * n_vars * count:
+            raise SbError(f"{w.size} witness bytes are not {count} witnesses of {n_vars} elements")
+    if count == 0:
+        return w, None, None, 0
+    r = np.frombuffer(b"".join(bytes(x[0]) for x in rs), np.uint8)
+    s = np.frombuffer(b"".join(bytes(x[1]) for x in rs), np.uint8)
+    if r.size != 32 * count or s.size != 32 * count:
+        raise SbError("r and s must be 32-byte Fr elements")
+    return w, r, s, count
+
+
+class KeyOnContexts:
+    """A zkey loaded on several contexts by one sb_<PROTO>_<LOAD> call.  curves are Curve objects of the key's curve
+    (several may be on one device) or device indices, for which the key makes its own Curve and closes it on release().
+    curves[0] is rank 0: errors of the multi-context calls are reported on it."""
+
+    PROTO, LOAD = "groth16", "load_replicas"
+    FIELDS = ("nVars", "nPublic", "domainSize")
+    read_header = staticmethod(read_zkey_header_groth16)
+
+    def __init__(self, zkey: bytes, curves):
+        zkey = bytes(zkey)
+        self.header = self.read_header(zkey)
+        if not curves:
+            raise SbError("at least one curve is needed")
+        self.curves, self._own, self.handles = [], [], None
+        try:
+            for c in curves:
+                if isinstance(c, int):
+                    c = getCurveFromQ(self.header["q"], c)
+                    self._own.append(c)
+                self.curves.append(c)
+            n = len(self.curves)
+            self._ctxs = (ctypes.c_void_p * n)(*[c.handle.value for c in self.curves])
+            handles = (ctypes.c_uint64 * n)()
+            buf = np.frombuffer(zkey, np.uint8)
+            c0 = self.curves[0]
+            c0.check(getattr(c0.lib, f"sb_{self.PROTO}_{self.LOAD}")(self._ctxs, n, _ptr(buf), buf.size, handles))
+            self.handles = handles
+        except BaseException:
+            self.release()
+            raise
+        for k in self.FIELDS:
+            setattr(self, k, self.header[k])
+
+    @property
+    def curve(self):
+        return self.curves[0]
+
+    def release(self):
+        if self.handles is not None:
+            for c, h in zip(self.curves, self.handles):
+                getattr(c.lib, f"sb_{self.PROTO}_release")(c.handle, h)
+            self.handles = None
+        for c in self._own:
+            c.terminate()
+        self._own = []
+
+
+class ReplicatedProvingKey(KeyOnContexts):
+    """A Groth16 zkey loaded whole on several contexts (sb_groth16_load_replicas), so that a batch of proofs is split
+    over them (sb_groth16_prove_batch_multi): context i proves a contiguous share of the batch."""
+
+    def prove_batch_raw(self, witnesses, rs) -> list:
+        """As ProvingKey.prove_batch_raw, over every context: the proofs are byte-identical to it."""
+        w, r, s, count = _batch_inputs(self.nVars, witnesses, rs)
+        if count == 0:
+            return []
+        c = self.curves[0]
+        pb = 8 * c.n8q
+        out = np.empty(count * pb, np.uint8)
+        c.check(c.lib.sb_groth16_prove_batch_multi(self._ctxs, self.handles, len(self.curves), _ptr(w), w.size // 32 // count, count,
+                                                   _ptr(r), _ptr(s), _ptr(out)))
+        return [out[i * pb:(i + 1) * pb].tobytes() for i in range(count)]
+
+
 class ProvingKey:
     """A Groth16 zkey registered on one device (bases + CSR coefficients resident in HBM)."""
 
@@ -143,25 +232,9 @@ class ProvingKey:
     def prove_batch_raw(self, witnesses, rs) -> list:
         """witnesses = a sequence of section-2 payloads (nVars * 32 bytes each) or one buffer of them back to back;
         rs = [(r, s), ...] one pair per witness -> affine proof bytes per witness, each equal to prove_raw's."""
-        count = len(rs)
-        if isinstance(witnesses, (list, tuple)):
-            if len(witnesses) != count:
-                raise SbError(f"{len(witnesses)} witnesses but {count} (r, s) pairs")
-            parts = [_arr(x) for x in witnesses]
-            for x in parts:
-                if x.size != 32 * self.nVars:
-                    raise SbError(f"Invalid witness length. Circuit: {self.nVars}, witness: {x.size // 32}")
-            w = np.concatenate(parts) if parts else np.zeros(0, np.uint8)
-        else:
-            w = _arr(witnesses)
-            if w.size != 32 * self.nVars * count:
-                raise SbError(f"{w.size} witness bytes are not {count} witnesses of {self.nVars} elements")
+        w, r, s, count = _batch_inputs(self.nVars, witnesses, rs)
         if count == 0:
             return []
-        r = np.frombuffer(b"".join(bytes(x[0]) for x in rs), np.uint8)
-        s = np.frombuffer(b"".join(bytes(x[1]) for x in rs), np.uint8)
-        if r.size != 32 * count or s.size != 32 * count:
-            raise SbError("r and s must be 32-byte Fr elements")
         pb = 8 * self.curve.n8q
         out = np.empty(count * pb, np.uint8)
         self.curve.check(self.curve.lib.sb_groth16_prove_batch(self.curve.handle, self.handle, _ptr(w), w.size // 32 // count, count,

@@ -12,7 +12,7 @@ import struct
 import numpy as np
 
 from .curve import Curve, SbError, _arr, _ptr, getCurveFromQ
-from .groth16 import _from_mont, random_fr, read_binfile, read_wtns_header
+from .groth16 import KeyOnContexts, _from_mont, random_fr, read_binfile, read_wtns_header
 
 POINTS = ("A", "B", "C", "Z", "T1", "T2", "T3", "Wxi", "Wxiw")
 EVALS = ("eval_a", "eval_b", "eval_c", "eval_s1", "eval_s2", "eval_zw")
@@ -47,6 +47,34 @@ def proof_to_object(curve: Curve, raw: bytes) -> dict:
     out["protocol"] = "plonk"
     out["curve"] = curve.name
     return out
+
+
+def _prove_batch(curve: Curve, proto: str, n_blinders: int, witnesses, blinders_list, call) -> list:
+    """prove_batch_raw of the PLONK and fflonk keys: checks the arguments, then call(witnesses, n_witness, count, blinders,
+    proofs, status) (pointers and sizes) makes the device call.  One proof (bytes) per witness, None for a proof the
+    reference would have rejected; SbError for argument and device errors."""
+    parts = [_arr(x) for x in witnesses]
+    count = len(parts)
+    if len(blinders_list) != count:
+        raise SbError("one blinder set per witness")
+    if count == 0:
+        return []
+    for b in blinders_list:
+        if len(b) != n_blinders * 32:
+            raise SbError(f"blinders must be {n_blinders} field elements")
+    n_wit = parts[0].size // 32
+    for x in parts:
+        if x.size != parts[0].size:
+            raise SbError("witnesses of one batch must have the same length")
+    w = np.concatenate(parts)
+    bl = np.frombuffer(b"".join(bytes(b) for b in blinders_list), np.uint8)
+    pb = getattr(curve.lib, f"sb_{proto}_proof_bytes")(curve.handle)
+    out = np.empty(count * pb, np.uint8)
+    status = np.zeros(count, np.int32)
+    rc = call(_ptr(w), n_wit, count, _ptr(bl), _ptr(out), _ptr(status))
+    if rc != 0 and not status.any():
+        curve.check(rc)
+    return [None if status[i] else out[i * pb:(i + 1) * pb].tobytes() for i in range(count)]
 
 
 class ProvingKey:
@@ -97,29 +125,8 @@ class ProvingKey:
         """One sb_plonk_prove_batch call: witnesses = wtns section-2 payloads ((nVars - nAdditions) x 32 bytes each),
         blinders_list = one 11 x 32-byte Montgomery blinder string per witness.  Returns one proof (bytes, as prove_raw) per
         witness, or None for a proof the reference would have rejected; raises SbError for argument and device errors."""
-        parts = [_arr(x) for x in witnesses]
-        count = len(parts)
-        if len(blinders_list) != count:
-            raise SbError("one blinder set per witness")
-        if count == 0:
-            return []
-        for b in blinders_list:
-            if len(b) != 11 * 32:
-                raise SbError("blinders must be 11 field elements")
-        n_wit = parts[0].size // 32
-        for x in parts:
-            if x.size != parts[0].size:
-                raise SbError("witnesses of one batch must have the same length")
-        lib, c = self.curve.lib, self.curve
-        w = np.concatenate(parts)
-        bl = np.frombuffer(b"".join(bytes(b) for b in blinders_list), np.uint8)
-        pb = lib.sb_plonk_proof_bytes(c.handle)
-        out = np.empty(count * pb, np.uint8)
-        status = np.zeros(count, np.int32)
-        rc = lib.sb_plonk_prove_batch(c.handle, self.handle, _ptr(w), n_wit, count, _ptr(bl), _ptr(out), _ptr(status))
-        if rc != 0 and not status.any():
-            c.check(rc)
-        return [None if status[i] else out[i * pb:(i + 1) * pb].tobytes() for i in range(count)]
+        return _prove_batch(self.curve, "plonk", 11, witnesses, blinders_list,
+                            lambda w, n_wit, count, bl, out, st: self.curve.lib.sb_plonk_prove_batch(self.curve.handle, self.handle, w, n_wit, count, bl, out, st))
 
     def release(self):
         if self.handle:
@@ -129,45 +136,17 @@ class ProvingKey:
             self.curve.terminate()
 
 
-class ShardedProvingKey:
+class ShardedProvingKey(KeyOnContexts):
     """A PLONK zkey spread over several contexts so that one proof uses all of them (sb_plonk_load_multi /
     sb_plonk_prove_multi).  curves[0] is rank 0: it holds the key and runs the proof; every context holds a contiguous
     range of the PTau points and computes that part of each commitment.  curves are Curve objects of the key's curve
     (several may be on one device) or device indices, for which the key makes its own Curve and closes it on release().
     Proofs are byte-identical to ProvingKey.prove_raw with the same witness and blinders."""
 
-    PROTO, N_BLINDERS = "plonk", 11
+    PROTO, LOAD, N_BLINDERS = "plonk", "load_multi", 11
+    FIELDS = ("nVars", "nPublic", "domainSize", "nAdditions")
     read_header = staticmethod(read_zkey_header_plonk)
     to_object = staticmethod(proof_to_object)
-
-    def __init__(self, zkey: bytes, curves):
-        zkey = bytes(zkey)
-        self.header = self.read_header(zkey)
-        if not curves:
-            raise SbError("at least one curve is needed")
-        self.curves, self._own, self.handles = [], [], None
-        try:
-            for c in curves:
-                if isinstance(c, int):
-                    c = getCurveFromQ(self.header["q"], c)
-                    self._own.append(c)
-                self.curves.append(c)
-            n = len(self.curves)
-            self._ctxs = (ctypes.c_void_p * n)(*[c.handle.value for c in self.curves])
-            handles = (ctypes.c_uint64 * n)()
-            buf = np.frombuffer(zkey, np.uint8)
-            c0 = self.curves[0]
-            c0.check(getattr(c0.lib, f"sb_{self.PROTO}_load_multi")(self._ctxs, n, _ptr(buf), buf.size, handles))
-            self.handles = handles
-        except BaseException:
-            self.release()
-            raise
-        for k in ("nVars", "nPublic", "domainSize", "nAdditions"):
-            setattr(self, k, self.header[k])
-
-    @property
-    def curve(self):
-        return self.curves[0]
 
     def prove_raw(self, witness, blinders: bytes) -> bytes:
         """witness = wtns section 2 ((nVars - nAdditions) x 32 bytes, plain LE); blinders = N_BLINDERS x 32 Montgomery bytes."""
@@ -193,14 +172,21 @@ class ShardedProvingKey:
         pub = [str(int.from_bytes(W[i * 32:(i + 1) * 32], "little")) for i in range(1, self.nPublic + 1)]
         return self.to_object(self.curve, raw), pub
 
-    def release(self):
-        if self.handles is not None:
-            for c, h in zip(self.curves, self.handles):
-                getattr(c.lib, f"sb_{self.PROTO}_release")(c.handle, h)
-            self.handles = None
-        for c in self._own:
-            c.terminate()
-        self._own = []
+
+class ReplicatedProvingKey(KeyOnContexts):
+    """A PLONK zkey loaded whole on several contexts (sb_plonk_load_replicas), so that a batch of proofs is split over
+    them (sb_plonk_prove_batch_multi): context i proves a contiguous share of the batch.  curves as for
+    ShardedProvingKey."""
+
+    PROTO, LOAD, N_BLINDERS = "plonk", "load_replicas", 11
+    FIELDS = ("nVars", "nPublic", "domainSize", "nAdditions")
+    read_header = staticmethod(read_zkey_header_plonk)
+
+    def prove_batch_raw(self, witnesses, blinders_list) -> list:
+        """As ProvingKey.prove_batch_raw, over every context: the proofs and statuses are those of one context's batch."""
+        fn = getattr(self.curve.lib, f"sb_{self.PROTO}_prove_batch_multi")
+        return _prove_batch(self.curve, self.PROTO, self.N_BLINDERS, witnesses, blinders_list,
+                            lambda w, n_wit, count, bl, out, st: fn(self._ctxs, self.handles, len(self.curves), w, n_wit, count, bl, out, st))
 
 
 def prove(zkey, wtns: bytes, blinders: bytes | None = None, logger=None, options=None):
