@@ -579,10 +579,8 @@ def fflonk_setup_synth(gates, additions, n_vars: int, n_public: int, tau: int, s
     for col, name in enumerate(("S1", "S2", "S3")):
         payload, polys[name] = p4(sigma[col * n:(col + 1) * n])
         secs.append((12 + col, payload))
-    payload = b""
-    for i in range(max(n_public, 1)):
-        payload += p4([1 if j == i else 0 for j in range(n)])[0]
-    secs.append((15, payload))
+    # joined once: appending to one bytes object is quadratic in n_public
+    secs.append((15, b"".join(p4([1 if j == i else 0 for j in range(n)])[0] for i in range(max(n_public, 1)))))
     npts = 9 * n + 18
     pts = _tau_powers(ci, tau, npts) if structured else bytes(orc.gen_points(ci.id, 1, tau & 0xFFFFFFFF, npts))
     secs.append((16, pts))

@@ -720,11 +720,8 @@ def plonk_setup_synth(gates, additions, n_vars: int, n_public: int, tau: int, st
         payload += pl
         header_pts[name] = commit_coef(coef)
     secs.append((12, payload))
-    payload = b""
-    for i in range(max(n_public, 1)):                                               # writeLs, plonk_setup.js:440-450
-        pl, _ = p4([1 if j == i else 0 for j in range(n)])
-        payload += pl
-    secs.append((13, payload))
+    # writeLs, plonk_setup.js:440-450 (joined once: appending to one bytes object is quadratic in n_public)
+    secs.append((13, b"".join(p4([1 if j == i else 0 for j in range(n)])[0] for i in range(max(n_public, 1)))))
     secs.append((14, pts))
     x2 = _g2_times_gen(ci, tau) if structured else ci.g2_affine_bytes(ci.g2)
     hdr = struct.pack("<I", ci.n8q) + ci.q.to_bytes(ci.n8q, "little") + struct.pack("<I", 32) + r.to_bytes(32, "little")

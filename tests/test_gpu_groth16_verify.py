@@ -84,10 +84,32 @@ def pub_bytes(s):
     return b"".join(v.to_bytes(32, "little") for v in s)
 
 
+def tampered_indices(n):
+    """The public indices whose tampering pool() tries: every one up to 300 inputs, else the ends and the middle."""
+    return range(n) if n <= 300 else sorted({0, 1, n // 2, n - 2, n - 1})
+
+
 def pool(f: Forged, m, seed):
-    """m forged (publics, proof, expected status) triples: valid and invalid, infinities, boundary signals."""
+    """m forged (publics, proof, expected status) triples: valid and invalid, infinities, boundary signals; then, on one
+    valid proof with distinct signals, three edits per index of tampered_indices: s_j + 1 (status 1, or 0 where IC[j+1] is
+    infinity), s_j = r (status 2) and s_j swapped with a neighbour (status 1: each signal must meet its own IC point)."""
     rng = random.Random(seed)
     r, out = f.r, []
+    if f.n:
+        s = [rng.randrange(r) for _ in range(f.n)]
+        prf = f.proof(s, rng.randrange(1, r), rng.randrange(1, r))
+        out.append((s, prf, 0))
+        for j in tampered_indices(f.n):
+            s1, s2 = list(s), list(s)
+            s1[j] = (s[j] + 1) % r
+            s2[j] = r
+            out += [(s1, prf, 0 if f.cp(s1) == f.cp(s) else 1), (s2, prf, 2)]
+            if f.n > 1:
+                i = j + 1 if j + 1 < f.n else j - 1
+                sw = list(s)
+                sw[i], sw[j] = s[j], s[i]
+                assert s[i] != s[j] and f.cp(sw) != f.cp(s)
+                out.append((sw, prf, 1))
     for i in range(m):
         kind = i % 8
         s = [rng.choice([0, 1, r - 1, rng.randrange(r)]) for _ in range(f.n)]
@@ -138,7 +160,7 @@ CURVE_IDS = [BN, BLS]
 
 
 @pytest.mark.parametrize("cid", CURVE_IDS, ids=["bn254", "bls12381"])
-@pytest.mark.parametrize("n_public", [0, 1, 2, 7, 64])
+@pytest.mark.parametrize("n_public", [0, 1, 2, 7, 64, 255, 256, 257, 1000, 4096])
 def test_forged_statuses(curves, cid, n_public):
     c = curves[cid]
     f = Forged(cid, n_public, seed=100 + n_public, zero_k=(0, 2) if n_public >= 2 else ())
@@ -197,6 +219,41 @@ def test_forged_batches(curves, cid, count, cap):
     want = [e for _s, _p, e in items]
     assert st == want, [i for i in range(count) if st[i] != want[i]][:10]
     assert c.last_ms(0) > 0
+
+
+# sb_groth16_verify_batch's sub-batch (api_verify.inl): min(count, VERIFY_CHUNK, VERIFY_BUDGET / per_proof)
+VERIFY_CHUNK, VERIFY_BUDGET = 1 << 15, 512 << 20
+
+
+@pytest.mark.parametrize("cid", CURVE_IDS, ids=["bn254", "bls12381"])
+def test_forged_budget_sub_batches(curves, cid):
+    """16384 public inputs: the 512 MiB budget, not the 2^15 chunk or a tuning cap, splits 2 chunk + 1 proofs into three
+    sub-batches (seen in the launch count), and the proofs on both sides of each split get their own statuses."""
+    c = curves[cid]
+    n8, n = c.n8q, 16384
+    per_proof = 8 * n8 + n * (32 + 4 * n8) + 4           # proof, publics, their XYZZ terms, status
+    chunk = VERIFY_BUDGET // per_proof
+    count = 2 * chunk + 1
+    assert chunk < count < VERIFY_CHUNK
+    f = Forged(cid, n, seed=41)
+    rng = random.Random(41)
+    valid = []
+    for _ in range(4):
+        s = [rng.randrange(f.r) for _ in range(n)]
+        valid.append((s, f.proof(s, rng.randrange(1, f.r), rng.randrange(1, f.r)), 0))
+    s, prf, _ = valid[0]
+    edits = {chunk - 1: (n - 1, f.r, 2), chunk: (n - 1, (s[n - 1] + 1) % f.r, 1), 2 * chunk - 1: (0, (s[0] + 1) % f.r, 1),
+             2 * chunk: (0, f.r, 2)}
+    items = [valid[rng.randrange(4)] for _ in range(count)]
+    for k, (j, v, want) in edits.items():
+        items[k] = (s[:j] + [v] + s[j + 1:], prf, want)
+    lib = c.lib
+    assert lib.sb_set_tuning(14, 0) == 0
+    before = lib.sb_launch_count(c.handle)
+    st = run_items(c, f, items)
+    assert lib.sb_launch_count(c.handle) - before == 1 + 3 * 2     # prepare, then terms and verify per sub-batch
+    assert [st[k] for k in sorted(edits)] == [edits[k][2] for k in sorted(edits)]
+    assert st == [e for _s, _p, e in items]
 
 
 @pytest.mark.parametrize("cid", CURVE_IDS, ids=["bn254", "bls12381"])

@@ -2,10 +2,12 @@
 fflonk.verify / verify_batch.
 
 Proofs come from the device provers: on the reference's fixture keys they verify under the reference's vk.json and
-public.json; on the synthetic keys of test_gpu_plonk_batch.py (BLS12-381 and 5 public inputs included) whole prove_batch
-batches verify.  Every status is provoked at its reference priority by editing proof bytes through the ABI, and a sample of
-distinct items is compared with the oracle's verifiers on the wrapper-decoded proof, including BLS12-381 commitments that
-are on the curve but outside the r-subgroup.  Large batches repeat a checked pool, so every expected status is known."""
+public.json; on the synthetic keys of test_gpu_plonk_batch.py (BLS12-381 and 5 public inputs included), and on keys whose
+public signals end the first Keccak absorb on a block boundary or number 1000, whole prove_batch batches verify.  Every
+status is provoked at its reference priority by editing proof bytes through the ABI (every public index included), and a
+sample of distinct items is compared with the oracle's verifiers on the wrapper-decoded proof, including BLS12-381
+commitments that are on the curve but outside the r-subgroup.  Large batches repeat a checked pool, so every expected
+status is known; at 1000 public signals the per-proof memory budget, not the proof count, splits them into sub-batches."""
 import contextlib
 import ctypes
 import functools
@@ -26,9 +28,15 @@ from oracle import plonk as OP  # noqa: E402
 BN, BLS = O.BN254, O.BLS12_381
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SB_ERR_ARG = -1
-# label: (protocol, curve, gates, public inputs)
+# label: (protocol, curve, gates, public inputs).  The rate labels put the first challenge's absorb on a whole number of
+# Keccak blocks, so its padding takes a block of its own; the pub1000 labels run the per-proof public-input loops (PI(xi)
+# and the transcript) far past the small counts.
 SYNTH = {"plonk-g13": ("plonk", BN, 13, 1), "plonk-pub5": ("plonk", BN, 60, 5), "plonk-bls": ("plonk", BLS, 120, 1),
-         "plonk-bls-pub5": ("plonk", BLS, 29, 5), "fflonk-g13": ("fflonk", BN, 13, 1), "fflonk-pub5": ("fflonk", BN, 60, 5)}
+         "plonk-bls-pub5": ("plonk", BLS, 29, 5), "fflonk-g13": ("fflonk", BN, 13, 1), "fflonk-pub5": ("fflonk", BN, 60, 5),
+         "plonk-rate12": ("plonk", BN, 60, 12), "plonk-bls-rate18": ("plonk", BLS, 60, 18), "fflonk-rate13": ("fflonk", BN, 60, 13),
+         "plonk-pub1000": ("plonk", BN, 3000, 1000), "plonk-bls-pub1000": ("plonk", BLS, 3000, 1000),
+         "fflonk-pub1000": ("fflonk", BN, 3000, 1000)}
+KECCAK_RATE = 136
 
 
 @pytest.fixture(scope="module")
@@ -103,6 +111,18 @@ def test_reference_fixtures(curves):
     (fproof, fp2), = prove(curves, "fflonk", BN, f["zkey"], f["wtns"], 1)
     assert fp2 == fpub
     assert mod("fflonk").verify(fvk, fpub, fproof, curve=curves[BN])
+
+
+def first_absorb(proto, cid, n_pub):
+    """Bytes absorbed before the first challenge: PLONK's 8 key points, the publics and A, B, C; fflonk's C0, the publics
+    and C1 (points uncompressed, signals 32 bytes)."""
+    return (11 if proto == "plonk" else 2) * 2 * O.CURVES[cid].n8q + 32 * n_pub
+
+
+@pytest.mark.parametrize("label", ["plonk-bls", "plonk-rate12", "plonk-bls-rate18", "fflonk-rate13"])
+def test_rate_labels_fill_whole_keccak_blocks(label):
+    proto, cid, _g, n_pub = SYNTH[label]
+    assert first_absorb(proto, cid, n_pub) % KECCAK_RATE == 0
 
 
 @pytest.mark.parametrize("label", list(SYNTH))
@@ -247,6 +267,42 @@ def test_large_batches_across_sub_batches(curves, label):
         assert rc == 0
         assert st == [items[i][2] for i in order], (cap, count)
         assert c.lib.sb_last_ms(c.handle, 0) > 0
+
+
+# the verify entries' sub-batch (api_verify.inl): min(count, VERIFY_CHUNK, VERIFY_BUDGET / per_proof); the scalars and
+# point terms per proof (verify_plonk.cuh): PLONK 18 and 17, fflonk 5 and 5; launches per sub-batch: PLONK 4, fflonk 3
+VERIFY_CHUNK, VERIFY_BUDGET = 1 << 15, 512 << 20
+PV_SHAPE = {"plonk": (18, 17, 4), "fflonk": (5, 5, 3)}
+
+
+@pytest.mark.parametrize("label", ["plonk-pub1000", "fflonk-pub1000"])
+def test_budget_sub_batches(curves, label):
+    """1000 public inputs: the 512 MiB budget, not the 2^15 chunk or a tuning cap, splits 2 chunk + 1 proofs into three
+    sub-batches (seen in the launch count); tampered signals at the last and first index sit on both sides of each split."""
+    proto, cid, _g, n_pub = SYNTH[label]
+    c = curves[cid]
+    vkb, n_pub, power, items = pool(label)
+    n_sc, n_terms, launches = PV_SHAPE[proto]
+    pb, prf, _ = items[0]
+    per_proof = len(prf) + 32 * n_pub + 32 * n_sc + n_terms * 4 * c.n8q + 4     # proof, publics, scalars, XYZZ terms, status
+    chunk = VERIFY_BUDGET // per_proof
+    count = 2 * chunk + 1
+    assert chunk < count < VERIFY_CHUNK
+    r = O.CURVES[cid].r
+    sig = lambda j, v: pb[:32 * j] + v.to_bytes(32, "little") + pb[32 * (j + 1):]
+    last, first = int.from_bytes(pb[-32:], "little"), int.from_bytes(pb[:32], "little")
+    edits = {chunk - 1: (sig(n_pub - 1, r), prf, 2), chunk: (sig(n_pub - 1, (last + 1) % r), prf, 1),
+             2 * chunk - 1: (sig(0, (first + 1) % r), prf, 1), 2 * chunk: (sig(0, r), prf, 2)}
+    valid = [it for it in items if it[2] == 0]
+    rng = random.Random(13)
+    order = [edits[k] if k in edits else valid[rng.randrange(len(valid))] for k in range(count)]
+    before = c.lib.sb_launch_count(c.handle)
+    with batch_cap(c.lib, 0):
+        rc, st = raw(c, proto, vkb, n_pub, power, b"".join(i[0] for i in order), b"".join(i[1] for i in order), count)
+    assert rc == 0
+    assert c.lib.sb_launch_count(c.handle) - before == 1 + 3 * launches     # prepare, then each sub-batch's kernels
+    assert [st[k] for k in sorted(edits)] == [edits[k][2] for k in sorted(edits)]
+    assert st == [i[2] for i in order]
 
 
 def test_batch_of_one_equals_verify_and_count_zero(curves):

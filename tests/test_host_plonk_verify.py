@@ -185,9 +185,9 @@ def _golden(name):
     return {k: bytes(g[k]) for k in g.files}
 
 
-def _synth(proto, n_pub, cid=O.BN254):
+def _synth(proto, n_pub, cid=O.BN254, n_gates=13):
     ci = O.CURVES[cid]
-    gates, adds, n_vars, npub, wit = OP.chain_gates(13, r=ci.r, n_pub=n_pub)
+    gates, adds, n_vars, npub, wit = OP.chain_gates(n_gates, r=ci.r, n_pub=n_pub)
     if proto == "plonk":
         zkey = OP.plonk_setup_synth(gates, adds, n_vars, npub, tau=0x5151 + n_pub, curve=cid)
     else:
@@ -201,6 +201,10 @@ def _plonk_cases():
     for n_pub in (1, 5):
         yield f"synth-pub{n_pub}", O.BN254, *_synth("plonk", n_pub)
     yield "synth-bls-pub5", O.BLS12_381, *_synth("plonk", 5, O.BLS12_381)
+    # the first challenge absorbs 704 + 32 n bytes on BN254 and 1056 + 32 n on BLS12-381: whole Keccak blocks at 12 and 18
+    yield "synth-pub12", O.BN254, *_synth("plonk", 12, n_gates=60)
+    yield "synth-bls-pub18", O.BLS12_381, *_synth("plonk", 18, O.BLS12_381, n_gates=60)
+    yield "synth-pub1000", O.BN254, *_synth("plonk", 1000, n_gates=3000)
 
 
 def _off_subgroup_point(rng):
@@ -247,6 +251,8 @@ def test_plonk_scalars_and_pairing_inputs(exe, tmp_path):
 def test_fflonk_scalars_and_pairing_inputs(exe, tmp_path):
     g = _golden("fflonk_case.npz")
     cases = [("fflonk_case", g["zkey"], g["wtns"])] + [(f"synth-pub{n}", *_synth("fflonk", n)) for n in (1, 5)]
+    # the first challenge absorbs C0, the publics and C1, 128 + 32 n bytes: whole Keccak blocks at 13
+    cases += [(f"synth-pub{n}", *_synth("fflonk", n, n_gates=ng)) for n, ng in ((13, 60), (1000, 3000))]
     recs, exp = [], []
     ci = O.CURVES[O.BN254]
     for label, zkey, wtns in cases:
